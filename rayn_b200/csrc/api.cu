@@ -73,7 +73,7 @@ struct RaynContext {
   int* d_batch_prefix = nullptr;  // [alloc_tiles + 1]
   int* d_work_ctr = nullptr;      // [WC_TOTAL] global work counters of the persistent kernels
   int n_sm = 148;
-  int occ_ext[SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT];
+  int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT];  // occ_ext[constant threshold][variant]
   int occ_pre = 8, occ_post = 8, occ_sph = 8;  // resident CTAs per SM of the work-list kernels
   int sdf_var[RAYN_MAX_HITABLES];  // march-kernel variant of every SDF hitable of the uploaded scene (rt_sdf2.cuh::sdf_variant)
   struct Div3Check { float min_r2, fixed_r2; bool ok; };
@@ -345,7 +345,8 @@ int32_t rayn_b200_create(const RaynConfig* cfg, RaynContext** out_ctx) {
   if (e == cudaSuccess) e = cudaEventCreate(&ctx->ev1);
   // persistent kernels: exactly as many CTAs as can be resident (one wave), so every CTA pulls work until the pass is drained
   for (int v = 0; v < SDFV_COUNT && e == cudaSuccess; ++v) {
-    DISPATCH_SDFV(v, e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[v], k_extend_march<V>, EXT_T, 0);
+    DISPATCH_SDFV(v, e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[0][v], k_extend_march<V, false>, EXT_T, 0);
+                  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[1][v], k_extend_march<V, true>, EXT_T, 0);
                   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_shd[v], k_shadow<V>, SHD_T, 0);
                   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_nrm[v], k_normals<V>, SLOT_BLOCK, 0));
   }
@@ -739,7 +740,11 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
             if (n_march++ > 0) CU(cudaMemsetAsync(ctx->d_work_ctr + WC_EXTEND, 0, sizeof(int), st));
             const int v = ctx->sdf_var[e];
             timed_begin(ctx, RAYN_K_EXTEND);
-            DISPATCH_SDFV(v, (k_extend_march<V><<<ctx->n_sm * ctx->occ_ext[v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, fold_all ? 1 : 0, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)));
+            const int sf = fold_all ? 1 : 0;
+            if (thr.is_const)
+              DISPATCH_SDFV(v, (k_extend_march<V, true><<<ctx->n_sm * ctx->occ_ext[1][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
+            else
+              DISPATCH_SDFV(v, (k_extend_march<V, false><<<ctx->n_sm * ctx->occ_ext[0][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
             timed_end(ctx, RAYN_K_EXTEND);
             ++e;
           }

@@ -449,8 +449,8 @@ __global__ void __launch_bounds__(EXT_BATCH) k_extend_spheres(const __grid_const
 // ------------------------------------------------------------------------------------------
 // K2 sphere-march: TracedSDF::hit (sdf.rs:59-83, SURVEY §9.1) for SDF hitable `hk` over every live
 // ray of the pass.  Persistent kernel: one wave of CTAs, warps pull 128-ray batches from a global
-// counter.  Each THREAD marches TWO rays ("slots"); their state lives in float2 registers (component
-// .x = slot 0, .y = slot 1) so every step of the distance estimator issues two independent operations (rt_sdf2.cuh).
+// counter.  Each THREAD marches TWO rays ("slots", MarchSlot below) whose points go through the distance estimator together,
+// so every step of it issues two independent operations (rt_sdf2.cuh).
 // One loop trip = one distance evaluation on every busy slot of the warp; a slot whose march ended is
 // refilled at the top of the next trip, so (nearly) all 64 slots of a warp evaluate every trip.  A march
 // depends only on its own ray, so the order in which slots pick up work cannot change any output bit.
@@ -479,7 +479,63 @@ __global__ void __launch_bounds__(EXT_BATCH) k_extend_spheres(const __grid_const
 #define RAYN_MARCH_OCC_BULB RAYN_MARCH_OCC  // same for the authored Mandelbulb estimator (needs more registers; tuning hook)
 #endif
 #define MARCH_OCC(V) ((V) == SDFV_BULB ? RAYN_MARCH_OCC_BULB : RAYN_MARCH_OCC)
-template <int V>
+// One march slot (two per thread).  Plain float registers: Hopper has no packed FP32 arithmetic, so the two slots gain
+// nothing from sharing 64-bit register pairs, and separate registers let ptxas load a float4 straight into a slot's state.
+// The point of the next evaluation is part of the state: the refill sets it to the origin (dist(origin), sdf.rs:30,60) and
+// every step that continues the march moves it to point_at(t) (ray.rs:22-24, sdf.rs:45: dir.mul_add(t, origin)), so no
+// trip selects between the two.  t starts at -0, which makes the first update `t + dist` exactly `dist` for every dist
+// (x + -0 = x, also for x = +-0 and NaN) without a select; steps < 0 still marks the first evaluation, which has no hit test.
+struct MarchSlot {
+  float ox, oy, oz, dx, dy, dz;  // ray origin (segment start) and direction
+  float px, py, pz;              // point of the next distance evaluation
+  float t, t_max;                // march distance; bound (closest hit so far / segment length)
+  int id, steps;                 // id < 0: empty; steps = evaluations after the first (-1 before it)
+};
+RT_D void slot_start(MarchSlot& s, float4 o, float4 d, float t_max) {
+  s.ox = o.x, s.oy = o.y, s.oz = o.z, s.dx = d.x, s.dy = d.y, s.dz = d.z;
+  s.px = o.x, s.py = o.y, s.pz = o.z;
+  s.t = -0.0f, s.t_max = t_max, s.steps = -1;
+}
+RT_D void slot_advance(MarchSlot& s) {
+  s.px = dm::mul_add(s.dx, s.t, s.ox), s.py = dm::mul_add(s.dy, s.t, s.oy), s.pz = dm::mul_add(s.dz, s.t, s.oz);
+}
+// an empty slot in the tail of a kernel evaluates a far point: cheapest for every estimator (the Mandelbulb leaves its loop
+// at once and counts no iteration)
+RT_D void slot_park(MarchSlot& s) { s.px = 100.0f, s.py = 0.0f, s.pz = 0.0f; }
+RT_D MarchSlot slot_empty() {
+  MarchSlot s;
+  slot_start(s, make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f), 0.0f);
+  s.id = -1;
+  return s;
+}
+
+// One step of TracedSDF::hit (sdf.rs:60-80) on one slot after its evaluation returned d.  Returns whether the march ended;
+// *hit = it ended on the hit test, with t unchanged.
+//   first evaluation (sdf.rs:60-61): t = dist(origin), no hit test;
+//   later (sdf.rs:65-80): hit when |dist| < max(0.00005 S, 0.05 S threshold(t)), else t += dist.
+//   max(c0, x) = (c0 < x ? x : c0): |d| < max(c0, x) <=> |d| < c0 || |d| < x.  For a NaN c0 (NaN S) the reference's max is NaN
+//   and nothing ever hits; then c1 and x are NaN as well, so both comparisons here are false too.
+//   The march also ends when t is NaN (a NaN t never satisfies hit or t > t_max again: the reference marches it to exhaustion
+//   and returns the same NaN) or after max_marches steps.
+// Dead evaluation: the reference tests t > t_max with the t from BEFORE the evaluation and then freezes t, whatever dist it
+// got (sdf.rs:65-80, merge on gt_mask).  So once an update makes t > t_max, the next evaluation cannot change the returned t;
+// the march ends right at that update, with that t, and the evaluation is not run.  Every slot that continues therefore has
+// t <= t_max (or a NaN t_max, for which t > t_max is never true), and the test on the old t is always false.  This holds for
+// every estimator and fold mode: the returned t is the reference's, and t > t_max is rejected by the fold at the end.
+template <bool THR_CONST>
+RT_D bool extend_step(MarchSlot& s, float d, float c0, float c1, float thr_scale, int max_marches, bool* hit) {
+  const float th = THR_CONST ? c1 : __fmul_rn(c1, __fmul_rn(thr_scale, s.t));  // THR_CONST: c1 is already 0.05 S scale
+  const float ad = dm::abs(d);
+  const bool h = (s.steps >= 0) && ((ad < c0) || (ad < th));  // side-effect free: predicate logic, no branches
+  const float tn = __fadd_rn(s.t, d);
+  const int sn = s.steps + 1;
+  s.t = h ? s.t : tn;
+  s.steps = h ? s.steps : sn;
+  *hit = h;
+  return h | (tn != tn) | (sn >= max_marches) | (tn > s.t_max);
+}
+
+template <int V, bool THR_CONST>
 __global__ void __launch_bounds__(EXT_T, MARCH_OCC(V)) k_extend_march(const __grid_constant__ DevScene sc, const PassBufs pb, const Thr thr,
                                                           const int hk, const int spheres_first, const int* __restrict__ batch_prefix,
                                                           int* __restrict__ work_ctr) {
@@ -487,20 +543,19 @@ __global__ void __launch_bounds__(EXT_T, MARCH_OCC(V)) k_extend_march(const __gr
   const int lane = threadIdx.x & 31;
   const unsigned lt = (1u << lane) - 1u;
   const float S = sc.rc.sdf_detail_scale;
-  const float c0 = 0.00005f * S, c1 = 0.05f * S;
-  const bool c0_num = c0 == c0;  // max(c0, x) of the reference is NaN for a NaN c0: nothing ever "hits"
+  const float c0 = 0.00005f * S;
+  // threshold(t) = scale * t, or the constant scale of an orthographic camera at depth 0 (camera.rs:282-284), a template
+  // parameter so that the choice is not made per trip
+  const float c1 = THR_CONST ? (0.05f * S) * thr.scale : 0.05f * S;
   const int max_marches = sc.rc.max_marches;
   const int n_batches = batch_prefix[pb.n_tiles];
-  // slot state: g < 0 = empty; steps = -1 = the first evaluation (dist(origin), sdf.rs:60) is still to come.
-  // Component .x of every packed value belongs to slot 0, .y to slot 1.
-  pk2 ox = pk(0.0f, 0.0f), oy = ox, oz = ox, dx = ox, dy = ox, dz = ox;
-  float2 t = splat2(0.0f), closest = t;
-  int g0 = -1, g1 = -1, steps0 = -1, steps1 = -1, evals = 0, bulb_iters = 0, trips = 0;
+  MarchSlot s0 = slot_empty(), s1 = slot_empty();
+  int evals = 0, bulb_iters = 0, trips = 0;
   int cur_base = 0, cur_pos = 0, cur_end = 0;
   bool exhausted = false;
   while (true) {
-    if (!exhausted || cur_pos < cur_end) {
-      unsigned idle0 = __ballot_sync(0xffffffffu, g0 < 0), idle1 = __ballot_sync(0xffffffffu, g1 < 0);
+    if (!exhausted) {
+      unsigned idle0 = __ballot_sync(0xffffffffu, s0.id < 0), idle1 = __ballot_sync(0xffffffffu, s1.id < 0);
       while (idle0 | idle1) {
         if (cur_pos >= cur_end) {
           int b = 0;
@@ -522,83 +577,51 @@ __global__ void __launch_bounds__(EXT_T, MARCH_OCC(V)) k_extend_march(const __gr
         const int avail = cur_end - cur_pos;
         const int n0 = __popc(idle0);
         const int rank0 = __popc(idle0 & lt), rank1 = n0 + __popc(idle1 & lt);
-        if (g0 < 0 && rank0 < avail) {
-          g0 = cur_base + pb.q_live[cur_base + cur_pos + rank0];
-          const float4 o4 = pb.o_time[g0], d4 = pb.d_t[g0];
-          ox = pk_set_x(ox, o4.x), oy = pk_set_x(oy, o4.y), oz = pk_set_x(oz, o4.z);
-          dx = pk_set_x(dx, d4.x), dy = pk_set_x(dy, d4.y), dz = pk_set_x(dz, d4.z);
-          closest.x = d4.w, t.x = 0.0f, steps0 = -1;
+        if (s0.id < 0 && rank0 < avail) {
+          const int g = cur_base + pb.q_live[cur_base + cur_pos + rank0];
+          const float4 d4 = pb.d_t[g];
+          slot_start(s0, pb.o_time[g], d4, d4.w);
+          s0.id = g;
         }
-        if (g1 < 0 && rank1 < avail) {
-          g1 = cur_base + pb.q_live[cur_base + cur_pos + rank1];
-          const float4 o4 = pb.o_time[g1], d4 = pb.d_t[g1];
-          ox = pk_set_y(ox, o4.x), oy = pk_set_y(oy, o4.y), oz = pk_set_y(oz, o4.z);
-          dx = pk_set_y(dx, d4.x), dy = pk_set_y(dy, d4.y), dz = pk_set_y(dz, d4.z);
-          closest.y = d4.w, t.y = 0.0f, steps1 = -1;
+        if (s1.id < 0 && rank1 < avail) {
+          const int g = cur_base + pb.q_live[cur_base + cur_pos + rank1];
+          const float4 d4 = pb.d_t[g];
+          slot_start(s1, pb.o_time[g], d4, d4.w);
+          s1.id = g;
         }
         cur_pos += min(avail, n0 + __popc(idle1));
-        idle0 = __ballot_sync(0xffffffffu, g0 < 0), idle1 = __ballot_sync(0xffffffffu, g1 < 0);
+        idle0 = __ballot_sync(0xffffffffu, s0.id < 0), idle1 = __ballot_sync(0xffffffffu, s1.id < 0);
       }
     }
-    // while work remains every slot is busy here; slots stay empty only in the tail of the kernel, where they are parked on a
-    // far point (cheapest for every estimator: the Mandelbulb leaves its loop at once and counts no iteration)
+    // while work remains every slot is busy here; slots stay empty only in the tail of the kernel
     if (exhausted) {
-      if (!__any_sync(0xffffffffu, g0 >= 0 || g1 >= 0)) break;
-      if (g0 < 0) ox = pk_set_x(ox, 100.0f), oy = pk_set_x(oy, 0.0f), oz = pk_set_x(oz, 0.0f), steps0 = -1;
-      if (g1 < 0) ox = pk_set_y(ox, 100.0f), oy = pk_set_y(oy, 0.0f), oz = pk_set_y(oz, 0.0f), steps1 = -1;
+      if (!__any_sync(0xffffffffu, s0.id >= 0 || s1.id >= 0)) break;
+      if (s0.id < 0) slot_park(s0);
+      if (s1.id < 0) slot_park(s1);
     }
-    // evaluation point of each slot: the origin for the first evaluation (sdf.rs:60), ray.point_at(t) afterwards
-    // (ray.rs:22-24: dir.mul_add(t, origin))
-    const bool first0 = steps0 < 0, first1 = steps1 < 0;
-    const float2 o_x = un(ox), o_y = un(oy), o_z = un(oz);
-    float2 px = muladd2(un(dx), t, o_x), py = muladd2(un(dy), t, o_y), pz = muladd2(un(dz), t, o_z);
-    if (first0) px.x = o_x.x, py.x = o_y.x, pz.x = o_z.x;
-    if (first1) px.y = o_x.y, py.y = o_y.y, pz.y = o_z.y;
-    const float2 dd = sdf_dist2<V>(k, px, py, pz, bulb_iters);
+    const float2 dd = sdf_dist2<V>(k, f2(s0.px, s1.px), f2(s0.py, s1.py), f2(s0.pz, s1.pz), bulb_iters);
     ++trips;
-    // per-slot march step, branch-free up to the (rare) end of a march:
-    //   first evaluation (sdf.rs:60-61): t = dist(origin), no hit test; a NaN start ends the march (the caller's t < closest is false);
-    //   later (sdf.rs:65-80): stop on |dist| < max(0.00005 S, 0.05 S threshold(t)) or t > t_max, else t += dist; a NaN t can never
-    //   satisfy hit/gt again, the reference marches it to exhaustion and returns NaN - ending at once returns the same NaN.
-    //   max(c0, x) = (c0 < x ? x : c0): for a non-NaN c0, |d| < max(c0, x) <=> |d| < c0 || |d| < x  (x NaN: both sides |d| < c0).
-    const float2 th = mul2(splat2(c1), thr.is_const ? splat2(thr.scale) : mul2(splat2(thr.scale), t));
-    const float2 tsum = add2(t, dd);
-    // (bitwise & | on the predicates: no short-circuit branches in the per-trip path)
-    bool done0, done1, stop0, stop1;
-    {
-      const float ad = dm::abs(dd.x);
-      stop0 = !first0 & ((c0_num & ((ad < c0) | (ad < th.x))) | (t.x > closest.x));
-      const float tn = first0 ? dd.x : tsum.x;
-      const int sn = steps0 + 1;
-      t.x = stop0 ? t.x : tn;
-      steps0 = stop0 ? steps0 : sn;
-      done0 = stop0 | (tn != tn) | (sn >= max_marches);
-    }
-    {
-      const float ad = dm::abs(dd.y);
-      stop1 = !first1 & ((c0_num & ((ad < c0) | (ad < th.y))) | (t.y > closest.y));
-      const float tn = first1 ? dd.y : tsum.y;
-      const int sn = steps1 + 1;
-      t.y = stop1 ? t.y : tn;
-      steps1 = stop1 ? steps1 : sn;
-      done1 = stop1 | (tn != tn) | (sn >= max_marches);
-    }
+    bool hit0, hit1;
+    const bool done0 = extend_step<THR_CONST>(s0, dd.x, c0, c1, thr.scale, max_marches, &hit0);
+    const bool done1 = extend_step<THR_CONST>(s1, dd.y, c0, c1, thr.scale, max_marches, &hit1);
+    slot_advance(s0);  // unused when the march ended: the refill starts the next one at its origin
+    slot_advance(s1);
     if (done0 | done1) {
-      if (done0 & (g0 >= 0)) {
-        if (t.x < closest.x || (spheres_first && t.x == closest.x && pb.q_key[g0] > hk)) {  // hitable.rs:190-193 (+ tie rule above)
-          pb.d_t[g0].w = t.x;
-          pb.q_key[g0] = hk;
+      if (done0 && s0.id >= 0) {
+        if (s0.t < s0.t_max || (spheres_first && s0.t == s0.t_max && pb.q_key[s0.id] > hk)) {  // hitable.rs:190-193 (+ tie rule above)
+          pb.d_t[s0.id].w = s0.t;
+          pb.q_key[s0.id] = hk;
         }
-        evals += steps0 + (stop0 ? 2 : 1);  // distance evaluations this march took
-        g0 = -1;
+        evals += s0.steps + (hit0 ? 2 : 1);  // distance evaluations this march took
+        s0.id = -1;
       }
-      if (done1 & (g1 >= 0)) {
-        if (t.y < closest.y || (spheres_first && t.y == closest.y && pb.q_key[g1] > hk)) {
-          pb.d_t[g1].w = t.y;
-          pb.q_key[g1] = hk;
+      if (done1 && s1.id >= 0) {
+        if (s1.t < s1.t_max || (spheres_first && s1.t == s1.t_max && pb.q_key[s1.id] > hk)) {
+          pb.d_t[s1.id].w = s1.t;
+          pb.q_key[s1.id] = hk;
         }
-        evals += steps1 + (stop1 ? 2 : 1);
-        g1 = -1;
+        evals += s1.steps + (hit1 ? 2 : 1);
+        s1.id = -1;
       }
     }
   }
@@ -847,6 +870,22 @@ __global__ void __launch_bounds__(128, RAYN_SHADE_PRE_OCC) k_shade_pre(const __g
 // ------------------------------------------------------------------------------------------
 #define SHD_T 128
 #define SHD_BATCH 128
+// One step of TracedSDF::occluded (sdf.rs:30-55) on one slot (MarchSlot: t = -0 makes the first update dist(start)).
+//   first (sdf.rs:30-36): t = dist(start);   later (:40-55): occluded when |dist| < max(1e-4 S, 1e-5 S t), else t += dist;
+//   the march ends unoccluded when t is NaN, exceeds max_dist (t_max), or after MAX_VIS_MARCHES steps.  A NaN S makes every
+//   threshold NaN: nothing is occluded, as in the reference.  *occ = 1: occluded.
+//   The reference's max(a, x) = (a < x ? x : a) equals fmaxf(a, x) whenever a is not NaN (for a NaN x both give a; a +-0 tie
+//   cannot change |d| < max); a NaN a means a NaN S, and then x is NaN too, so both are NaN and nothing is occluded.  The
+//   first evaluation compares against -1, which no |d| is below.  An int flag, not a bool: ptxas kept the bools in bytes.
+RT_D bool shadow_step(MarchSlot& s, float d, float oc0, float oc1, int max_vis, int* occ) {
+  const bool o = dm::abs(d) < (s.steps >= 0 ? fmaxf(oc0, __fmul_rn(oc1, s.t)) : -1.0f);
+  const float tn = __fadd_rn(s.t, d);
+  s.t = tn;
+  s.steps = s.steps + 1;
+  *occ = o ? 1 : 0;
+  return o | (tn != tn) | (s.steps >= max_vis) | (tn > s.t_max);
+}
+
 template <int V>
 __global__ void __launch_bounds__(SHD_T, MARCH_OCC(V)) k_shadow(const __grid_constant__ DevScene sc, const PassBufs pb, const int hk, const int j,
                                                     int* __restrict__ work_ctr) {
@@ -858,17 +897,18 @@ __global__ void __launch_bounds__(SHD_T, MARCH_OCC(V)) k_shadow(const __grid_con
   const float4* __restrict__ seg_b = pb.seg_b + (size_t)j * pb.seg_cap;
   const float S = sc.rc.sdf_detail_scale;
   const float oc0 = 0.0001f * S, oc1 = 0.00001f * S;
-  const bool oc0_num = oc0 == oc0;  // see k_extend_march
   const int max_vis = sc.rc.max_vis_marches;
-  // slot state (see k_extend_march): own < 0 = empty, steps = -1 = dist(start) (sdf.rs:30) still to come
-  pk2 sx = pk(0.0f, 0.0f), sy = sx, sz = sx, dx = sx, dy = sx, dz = sx;
-  float2 t = splat2(0.0f), max_dist = t;
-  int own0 = -1, own1 = -1, steps0 = -1, steps1 = -1, evals = 0, bulb_iters = 0, trips = 0;
+  // slot state (see k_extend_march); id = owner path g << 4 | light-sample bit
+  MarchSlot s0 = slot_empty(), s1 = slot_empty();
+  int evals = 0, bulb_iters = 0, trips = 0;
   int cur_pos = 0, cur_end = 0;
+  // the current batch, set once per batch: a refill indexes it with a 32-bit offset instead of rebuilding seg_a + j * seg_cap
+  const float4* __restrict__ qa = seg_a;
+  const float4* __restrict__ qb = seg_b;
   bool exhausted = false;
   while (true) {
-    if (!exhausted || cur_pos < cur_end) {
-      unsigned idle0 = __ballot_sync(0xffffffffu, own0 < 0), idle1 = __ballot_sync(0xffffffffu, own1 < 0);
+    if (!exhausted) {
+      unsigned idle0 = __ballot_sync(0xffffffffu, s0.id < 0), idle1 = __ballot_sync(0xffffffffu, s1.id < 0);
       while (idle0 | idle1) {
         if (cur_pos >= cur_end) {
           int b = 0;
@@ -878,74 +918,49 @@ __global__ void __launch_bounds__(SHD_T, MARCH_OCC(V)) k_shadow(const __grid_con
             exhausted = true;
             break;
           }
-          cur_pos = b;
-          cur_end = min(b + SHD_BATCH, n_seg);
+          qa = seg_a + b, qb = seg_b + b;
+          cur_pos = 0;
+          cur_end = min(SHD_BATCH, n_seg - b);
         }
         const int avail = cur_end - cur_pos;
         const int n0 = __popc(idle0);
         const int rank0 = __popc(idle0 & lt), rank1 = n0 + __popc(idle1 & lt);
-        if (own0 < 0 && rank0 < avail) {
-          const float4 a = seg_a[cur_pos + rank0], b4 = seg_b[cur_pos + rank0];
-          sx = pk_set_x(sx, a.x), sy = pk_set_x(sy, a.y), sz = pk_set_x(sz, a.z);
-          dx = pk_set_x(dx, b4.x), dy = pk_set_x(dy, b4.y), dz = pk_set_x(dz, b4.z);
-          max_dist.x = a.w, t.x = 0.0f, steps0 = -1;
-          own0 = __float_as_int(b4.w);
+        if (s0.id < 0 && rank0 < avail) {
+          const float4 a = qa[cur_pos + rank0], b4 = qb[cur_pos + rank0];
+          slot_start(s0, a, b4, a.w);
+          s0.id = __float_as_int(b4.w);
         }
-        if (own1 < 0 && rank1 < avail) {
-          const float4 a = seg_a[cur_pos + rank1], b4 = seg_b[cur_pos + rank1];
-          sx = pk_set_y(sx, a.x), sy = pk_set_y(sy, a.y), sz = pk_set_y(sz, a.z);
-          dx = pk_set_y(dx, b4.x), dy = pk_set_y(dy, b4.y), dz = pk_set_y(dz, b4.z);
-          max_dist.y = a.w, t.y = 0.0f, steps1 = -1;
-          own1 = __float_as_int(b4.w);
+        if (s1.id < 0 && rank1 < avail) {
+          const float4 a = qa[cur_pos + rank1], b4 = qb[cur_pos + rank1];
+          slot_start(s1, a, b4, a.w);
+          s1.id = __float_as_int(b4.w);
         }
         cur_pos += min(avail, n0 + __popc(idle1));
-        idle0 = __ballot_sync(0xffffffffu, own0 < 0), idle1 = __ballot_sync(0xffffffffu, own1 < 0);
+        idle0 = __ballot_sync(0xffffffffu, s0.id < 0), idle1 = __ballot_sync(0xffffffffu, s1.id < 0);
       }
     }
     if (exhausted) {  // tail of the kernel: empty slots are parked on a far point (see k_extend_march)
-      if (!__any_sync(0xffffffffu, own0 >= 0 || own1 >= 0)) break;
-      if (own0 < 0) sx = pk_set_x(sx, 100.0f), sy = pk_set_x(sy, 0.0f), sz = pk_set_x(sz, 0.0f), steps0 = -1;
-      if (own1 < 0) sx = pk_set_y(sx, 100.0f), sy = pk_set_y(sy, 0.0f), sz = pk_set_y(sz, 0.0f), steps1 = -1;
+      if (!__any_sync(0xffffffffu, s0.id >= 0 || s1.id >= 0)) break;
+      if (s0.id < 0) slot_park(s0);
+      if (s1.id < 0) slot_park(s1);
     }
-    const bool first0 = steps0 < 0, first1 = steps1 < 0;
-    const float2 s_x = un(sx), s_y = un(sy), s_z = un(sz);
-    float2 px = muladd2(un(dx), t, s_x), py = muladd2(un(dy), t, s_y), pz = muladd2(un(dz), t, s_z);  // dir.mul_add(t, start), sdf.rs:45
-    if (first0) px.x = s_x.x, py.x = s_y.x, pz.x = s_z.x;                                                                  // dist(start), sdf.rs:30
-    if (first1) px.y = s_x.y, py.y = s_y.y, pz.y = s_z.y;
-    const float2 dd = sdf_dist2<V>(k, px, py, pz, bulb_iters);
+    const float2 dd = sdf_dist2<V>(k, f2(s0.px, s1.px), f2(s0.py, s1.py), f2(s0.pz, s1.pz), bulb_iters);
     ++trips;
-    // per-slot step of TracedSDF::occluded, branch-free up to the end of a march (see k_extend_march):
-    //   first (sdf.rs:30-36): t = dist(start);   later (:40-55): occluded when |dist| < max(1e-4 S, 1e-5 S t), else t += dist;
-    //   the march ends unoccluded when t is NaN, exceeds max_dist, or after MAX_VIS_MARCHES steps.
-    const float2 th = mul2(splat2(oc1), t);
-    const float2 tsum = add2(t, dd);
-    bool done0, done1, occ0, occ1;
-    {
-      const float ad = dm::abs(dd.x);
-      occ0 = !first0 & oc0_num & ((ad < oc0) | (ad < th.x));
-      const float tn = first0 ? dd.x : tsum.x;
-      t.x = tn;
-      steps0 = steps0 + 1;
-      done0 = occ0 | (tn != tn) | (steps0 >= max_vis) | (tn > max_dist.x);
-    }
-    {
-      const float ad = dm::abs(dd.y);
-      occ1 = !first1 & oc0_num & ((ad < oc0) | (ad < th.y));
-      const float tn = first1 ? dd.y : tsum.y;
-      t.y = tn;
-      steps1 = steps1 + 1;
-      done1 = occ1 | (tn != tn) | (steps1 >= max_vis) | (tn > max_dist.y);
-    }
+    int occ0, occ1;
+    const bool done0 = shadow_step(s0, dd.x, oc0, oc1, max_vis, &occ0);
+    const bool done1 = shadow_step(s1, dd.y, oc0, oc1, max_vis, &occ1);
+    slot_advance(s0);  // dir.mul_add(t, start), sdf.rs:45
+    slot_advance(s1);
     if (done0 | done1) {
-      if (done0 & (own0 >= 0)) {
-        if (occ0) atomicAnd(pb.vis + ((unsigned)own0 >> 4), ~(1u << (own0 & 15)));
-        evals += steps0 + 1;  // distance evaluations this march took
-        own0 = -1;
+      if (done0 && s0.id >= 0) {
+        if (occ0) atomicAnd(pb.vis + ((unsigned)s0.id >> 4), ~(1u << (s0.id & 15)));
+        evals += s0.steps + 1;  // distance evaluations this march took
+        s0.id = -1;
       }
-      if (done1 & (own1 >= 0)) {
-        if (occ1) atomicAnd(pb.vis + ((unsigned)own1 >> 4), ~(1u << (own1 & 15)));
-        evals += steps1 + 1;
-        own1 = -1;
+      if (done1 && s1.id >= 0) {
+        if (occ1) atomicAnd(pb.vis + ((unsigned)s1.id >> 4), ~(1u << (s1.id & 15)));
+        evals += s1.steps + 1;
+        s1.id = -1;
       }
     }
   }
