@@ -350,6 +350,31 @@ typedef enum RaynPostMode {
 int32_t rayn_b200_film_postprocess(RaynContext* ctx, int32_t mode, int32_t width, int32_t height,
                                    const RaynFilmPlanes* planes, uint8_t* out, int32_t out_space);
 
+/* ---- film denoise: edge-avoiding a-trous wavelet filter (Dammertz et al., HPG 2010; PAPERS.md) -----------------
+ * Filters the color and background planes of a rendered film, guided by its normal and alpha planes, which the
+ * reference only writes out for an external denoiser (film.rs:326-372).  Level i = 0..iterations-1 uses step 2^i and
+ * the 5x5 taps q = p + 2^i (dx, dy), dx, dy in -2..2, kernel h = {1/16, 1/4, 3/8, 1/4, 1/16}; level 0 reads `in`,
+ * each later level reads the previous one, the last writes `out`.  Per tap, in float and in this order:
+ *   dc2 = (dr*dr + dg*dg) + db*db of c_q - c_p,  dn2 the same of n_q - n_p,  da2 = (a_q - a_p)^2
+ *   e = (dc2*ic_i + dn2*in) + da2*ia,  w = h[dy+2]*h[dx+2] * exp(-e)     (exp: detmath.h)
+ *   ic_i = ldexpf(1/(sigma_color^2), i),  in = 1/sigma_normal^2,  ia = 1/sigma_alpha^2
+ * output = (sum w*c_q) / (sum w), taps visited dy outer, dx inner, ascending.  Taps outside the image, taps with a
+ * non-finite colour component and taps whose e is NaN are skipped; a pixel whose own colour is non-finite is copied.
+ * A sigma must be > 0 (+inf disables its term) and large enough that every factor is finite; else
+ * RAYN_ERR_INVALID_ARG.  in->normal and in->alpha are required; in->color / in->background are optional, each one
+ * present needs the matching out plane.  out->color / out->background may be the same pointers as in's.
+ * in->space and out->space are RaynMemSpace each.  Device planes on both sides: asynchronous on the context's
+ * stream (rayn_b200_sync waits); otherwise the call copies, filters and returns with the result in place.
+ * Scratch is stream-ordered (cudaMallocAsync) and released within the call.                                    */
+typedef struct RaynDenoiseDesc {
+  int32_t iterations; /* levels L, 1..8 (step 2^i)               */
+  float sigma_color;  /* > 0; +inf disables the term             */
+  float sigma_normal;
+  float sigma_alpha;
+} RaynDenoiseDesc;
+int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* desc, int32_t width, int32_t height,
+                               const RaynFilmPlanes* in, const RaynFilmPlanes* out);
+
 /* ---- host-side input builders (pure CPU; stand in for crates the Rust host owns) ----
  * quasi-rd R_d tables (sampler.rs:18-37), rand SmallRng scramble (film.rs:460-461),
  * FilterImportanceSampler::new(BlackmanHarris) (filter.rs:13-49,196-218).               */

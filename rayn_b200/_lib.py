@@ -99,6 +99,10 @@ class RaynFilmPlanes(C.Structure):
                 ("normal", C.c_void_p), ("space", i32)]
 
 
+class RaynDenoiseDesc(C.Structure):
+    _fields_ = [("iterations", i32), ("sigma_color", f32), ("sigma_normal", f32), ("sigma_alpha", f32)]
+
+
 class RaynConfig(C.Structure):
     _fields_ = [("device", i32), ("max_paths_per_pass", i64), ("flags", i32)]
 
@@ -138,6 +142,7 @@ SYMBOLS = {
     "rayn_b200_film_pack_tiles": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(i32), i32, C.POINTER(RaynFilmPlanes), C.c_void_p]),
     "rayn_b200_film_unpack_tiles": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(i32), i32, C.c_void_p, C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_film_postprocess": (i32, [C.c_void_p, i32, i32, i32, C.POINTER(RaynFilmPlanes), C.c_void_p, i32]),
+    "rayn_b200_film_denoise": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_host_rd_tables": (i32, [i32, i32, i32, C.c_uint64, fp, fp]),
     "rayn_b200_host_scramble": (i32, [i32, i32, fp]),
     "rayn_b200_host_fis_blackman_harris": (i32, [f32, fp]),

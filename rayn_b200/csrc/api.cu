@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "rt_denoise.cuh"
 #include "rt_kernels.cuh"
 #ifdef RAYN_LEGACY_KERNELS
 #include "rt_legacy.cuh"
@@ -1195,6 +1196,88 @@ int32_t rayn_b200_film_postprocess(RaynContext* ctx, int32_t mode, int32_t W, in
   CU(cudaGetLastError());
   if (out_space == RAYN_MEM_HOST) CU(cudaMemcpyAsync(out, dout, nbytes, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  return RAYN_OK;
+}
+
+// ---- film denoise (rt_denoise.cuh; statement in include/rayn_b200.h) ----------------------------------------------
+// 1 / sigma^2 in float; +inf -> 0 (term disabled).  False for a sigma that is not > 0 or so small the factor overflows.
+static bool denoise_factor(float sigma, float* f) {
+  if (!(sigma > 0.0f)) return false;
+  *f = 1.0f / (sigma * sigma);
+  return isfinite(*f);
+}
+
+// Enqueues the whole filter on ctx->stream.  `scratch` holds guide + ping-pong planes (12 floats per pixel), then the
+// device copies of host-space inputs (10) and one host-space output channel (3), as the caller sized it.
+static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W, int H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
+                               float ic0, float in_, float ia, float* scratch) {
+  cudaStream_t st = ctx->stream;
+  const size_t npx = (size_t)W * H;
+  const unsigned blocks1d = (unsigned)((npx + 255) / 256);
+  float4* guide = (float4*)scratch;
+  float4* ping[2] = {guide + npx, guide + 2 * npx};
+  float* stage = scratch + 12 * npx;
+  const float *c_in = in->color, *b_in = in->background, *n_in = in->normal, *a_in = in->alpha;
+  if (in->space == RAYN_MEM_HOST) {
+    float* s = stage;
+    stage += 10 * npx;
+    CU(cudaMemcpyAsync(s, in->normal, npx * 12, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s + 3 * npx, in->alpha, npx * 4, cudaMemcpyHostToDevice, st));
+    if (in->color) CU(cudaMemcpyAsync(s + 4 * npx, in->color, npx * 12, cudaMemcpyHostToDevice, st));
+    if (in->background) CU(cudaMemcpyAsync(s + 7 * npx, in->background, npx * 12, cudaMemcpyHostToDevice, st));
+    n_in = s, a_in = s + 3 * npx, c_in = in->color ? s + 4 * npx : nullptr, b_in = in->background ? s + 7 * npx : nullptr;
+  }
+  k_denoise_guides<<<blocks1d, 256, 0, st>>>((long long)npx, n_in, a_in, guide);
+  CU(cudaGetLastError());
+  const dim3 blk(32, 8), grid((unsigned)((W + 31) / 32), (unsigned)((H + 7) / 8));
+  for (int ch = 0; ch < 2; ++ch) {
+    const float* src3 = ch == 0 ? c_in : b_in;
+    if (!src3) continue;
+    float* dst_user = ch == 0 ? out->color : out->background;
+    float* dst3 = out->space == RAYN_MEM_HOST ? stage : dst_user;
+    k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ping[0]);
+    for (int i = 0; i < d->iterations; ++i) {
+      const float ic = ldexpf(ic0, i);
+      const float4* src = ping[i & 1];
+      if (i == d->iterations - 1)
+        k_denoise_level<true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, nullptr, dst3);
+      else
+        k_denoise_level<false><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, ping[(i + 1) & 1], nullptr);
+    }
+    CU(cudaGetLastError());
+    if (out->space == RAYN_MEM_HOST) CU(cudaMemcpyAsync(dst_user, dst3, npx * 12, cudaMemcpyDeviceToHost, st));
+  }
+  return RAYN_OK;
+}
+
+int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                               const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!d || !in || !out || W <= 0 || H <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad argument");
+  if (d->iterations < 1 || d->iterations > 8) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: iterations %d not in [1,8]", d->iterations);
+  if (!in->normal || !in->alpha) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: the normal and alpha guide planes are required");
+  if ((in->color && !out->color) || (in->background && !out->background))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: every input colour plane needs its output plane");
+  if ((in->space != RAYN_MEM_HOST && in->space != RAYN_MEM_DEVICE) || (out->space != RAYN_MEM_HOST && out->space != RAYN_MEM_DEVICE))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad memory space");
+  float ic0, in_, ia;
+  if (!denoise_factor(d->sigma_color, &ic0) || !isfinite(ldexpf(ic0, d->iterations - 1)) || !denoise_factor(d->sigma_normal, &in_) ||
+      !denoise_factor(d->sigma_alpha, &ia))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: sigmas (%g, %g, %g) must be > 0 (+inf disables a term) and give finite 1/sigma^2",
+                d->sigma_color, d->sigma_normal, d->sigma_alpha);
+  CU(cudaSetDevice(ctx->device));
+  if (!in->color && !in->background) return RAYN_OK;
+  const size_t npx = (size_t)W * H;
+  const size_t nfloat = npx * (12 + (in->space == RAYN_MEM_HOST ? 10 : 0) + (out->space == RAYN_MEM_HOST ? 3 : 0));
+  cudaStream_t st = ctx->stream;
+  float* scratch = nullptr;
+  // stream-ordered and released below: nothing persists between calls (render-pass sizing reads cudaMemGetInfo)
+  CU(cudaMallocAsync((void**)&scratch, nfloat * sizeof(float), st));
+  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch);
+  const cudaError_t ef = cudaFreeAsync(scratch, st);
+  if (rc) return rc;
+  CU(ef);
+  if (in->space == RAYN_MEM_HOST || out->space == RAYN_MEM_HOST) CU(cudaStreamSynchronize(st));
   return RAYN_OK;
 }
 

@@ -1,0 +1,94 @@
+// rt_denoise.cuh — edge-avoiding a-trous wavelet filter of the film planes (Dammertz, Sewtz, Hanika, Lensch, HPG 2010).
+// The exact statement (tap order, the float arithmetic, which taps are skipped) is at rayn_b200_film_denoise in
+// include/rayn_b200.h; the CPU mirror in tests/denoise_oracle.cpp restates it and the GPU tests compare bit for bit.
+//
+// One kernel launch per level, one thread per pixel on 32x8 CTAs.  The guides are packed once into a float4
+// (nx, ny, nz, a) plane and the colour ping-pongs between two float4 planes, so every tap is two 16-byte loads that
+// mostly hit L1/L2 (neighbouring pixels share taps).
+#pragma once
+#include "rt_device.cuh"
+
+namespace rt {
+
+// Exact skip of dead taps.  dm::exp (detmath.h) returns +0 for every float argument x <= -103.972084f (bit pattern
+// 0xc2cff1b5); -103.972076f (0xc2cff1b4) is the lowest argument with a nonzero result (the smallest denormal).  This
+// is established on the device by tests/test_gpu_denoise.py, which evaluates dm::exp on every float in
+// [-111, -103.972084] and finds +0 for all of them; below -110 dm::exp clamps its argument to -110, so the sweep covers
+// every smaller argument too (including -inf).  Hence e > DENOISE_E_DEAD  =>  w = hk * exp(-e) = hk * (+0) = +0, and the
+// skipped update `s += (+0) * c_q` is the identity on every accumulator: c_q is finite (non-finite taps are skipped
+// first), so the product is +-0, and an accumulator that starts at +0 can never become -0 (round-to-nearest gives
+// x + (-x) = +0), so adding +-0 leaves its bits unchanged.  `!(e <= DENOISE_E_DEAD)` also catches e = NaN, a tap the
+// statement skips anyway.
+#define DENOISE_E_DEAD 103.972076f
+// e == 0 (identical colour and guides, always the centre tap) needs no exponential: dm::exp(-0.0f) is exactly 1.0f
+// (tested on both sides), so w = hk * 1 = hk.
+
+__device__ __forceinline__ bool dn_finite3(const float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z); }
+
+// planes -> float4 (r, g, b, 0) / (nx, ny, nz, a)
+__global__ void __launch_bounds__(256) k_denoise_pack(long long npx, const float* __restrict__ c3, float4* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npx) return;
+  out[i] = make_float4(c3[3 * i], c3[3 * i + 1], c3[3 * i + 2], 0.0f);
+}
+__global__ void __launch_bounds__(256) k_denoise_guides(long long npx, const float* __restrict__ n3, const float* __restrict__ a,
+                                                        float4* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npx) return;
+  out[i] = make_float4(n3[3 * i], n3[3 * i + 1], n3[3 * i + 2], a[i]);
+}
+
+// One level with step 2^level.  kOut3: the last level writes the interleaved rgb output plane instead of a float4 plane.
+template <bool kOut3>
+__global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, float ic, float in_, float ia, const float4* __restrict__ guide,
+                                                       const float4* __restrict__ src, float4* __restrict__ dst4, float* __restrict__ dst3) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= W || y >= H) return;
+  const size_t p = (size_t)y * W + x;
+  const float4 cp = src[p];
+  float4 o = cp;
+  if (dn_finite3(cp)) {
+    const float h[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
+    const float4 gp = guide[p];
+    float sr = 0.0f, sg = 0.0f, sb = 0.0f, sw = 0.0f;
+#pragma unroll
+    for (int dy = -2; dy <= 2; ++dy) {
+      const int qy = y + step * dy;
+      if (qy < 0 || qy >= H) continue;
+      const float4* srow = src + (size_t)qy * W;
+      const float4* grow = guide + (size_t)qy * W;
+#pragma unroll
+      for (int dx = -2; dx <= 2; ++dx) {
+        const int qx = x + step * dx;
+        if (qx < 0 || qx >= W) continue;
+        const float4 cq = srow[qx];
+        if (!dn_finite3(cq)) continue;
+        const float4 gq = grow[qx];
+        const float dr = cq.x - cp.x, dg = cq.y - cp.y, db = cq.z - cp.z;
+        const float dc2 = (dr * dr + dg * dg) + db * db;
+        const float nx = gq.x - gp.x, ny = gq.y - gp.y, nz = gq.z - gp.z;
+        const float dn2 = (nx * nx + ny * ny) + nz * nz;
+        const float da = gq.w - gp.w;
+        const float da2 = da * da;
+        const float e = (dc2 * ic + dn2 * in_) + da2 * ia;
+        if (!(e <= DENOISE_E_DEAD)) continue;  // NaN (skipped by the statement) or a weight of exactly +0 (argument above)
+        const float hk = h[dy + 2] * h[dx + 2];
+        const float w = e == 0.0f ? hk : hk * dm::exp(-e);
+        sr += w * cq.x;
+        sg += w * cq.y;
+        sb += w * cq.z;
+        sw += w;
+      }
+    }
+    o = make_float4(sr / sw, sg / sw, sb / sw, 0.0f);
+  }
+  if (kOut3) {
+    dst3[3 * p] = o.x;
+    dst3[3 * p + 1] = o.y;
+    dst3[3 * p + 2] = o.z;
+  } else {
+    dst4[p] = o;
+  }
+}
+
+}  // namespace rt

@@ -67,6 +67,18 @@ def make_frame_desc(width, height, tile_size, samples, integrator, frame, time_r
     return f
 
 
+# Picked by `tools/bench_denoise.py --pick-sigmas` (DESIGN.md §4b): the lowest col+bg MSE against a 256 spp film of a
+# 4 spp config 3 film at 96x96, 5 levels, over a grid of 9 x 6 x 4 sigmas.
+DENOISE_DEFAULTS = dict(sigma_color=2.5, sigma_normal=0.4, sigma_alpha=0.5)
+
+
+def denoise_desc(iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
+    """RaynDenoiseDesc; a sigma left None takes its DENOISE_DEFAULTS value."""
+    given = dict(sigma_color=sigma_color, sigma_normal=sigma_normal, sigma_alpha=sigma_alpha)
+    s = {k: float(DENOISE_DEFAULTS[k] if v is None else v) for k, v in given.items()}
+    return L.RaynDenoiseDesc(int(iterations), s["sigma_color"], s["sigma_normal"], s["sigma_alpha"])
+
+
 def tile_grid(width, height, tile_w, tile_h):
     nx, ny = C.c_int32(), C.c_int32()
     L.check(L.host_lib().rayn_b200_host_tile_grid(width, height, tile_w, tile_h, C.byref(nx), C.byref(ny)))
@@ -136,6 +148,24 @@ class Renderer:
         out = np.zeros((height, width, L.POST_BYTES[mode]), np.uint8)
         L.check(self._lib.rayn_b200_film_postprocess(self._ctx, mode, width, height, C.byref(p), out.ctypes.data, L.MEM_HOST), self._ctx)
         return out
+
+    def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
+        """Edge-avoiding a-trous filter of the color and background planes (include/rayn_b200.h: rayn_b200_film_denoise).
+        numpy planes in ("normal" and "alpha" required, "color" / "background" optional); returns new arrays for the
+        colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term."""
+        for k in ("normal", "alpha"):
+            if planes.get(k) is None:
+                raise ValueError(f"denoise needs the {k} guide plane")
+        flat = {k: np.ascontiguousarray(v, np.float32).reshape(-1) for k, v in planes.items() if v is not None}
+        outs = {k: np.empty_like(flat[k]) for k in ("color", "background") if k in flat}
+
+        def ptr(d, k):
+            return d[k].ctypes.data if k in d else None
+        pin = L.RaynFilmPlanes(ptr(flat, "color"), ptr(flat, "alpha"), ptr(flat, "background"), ptr(flat, "normal"), L.MEM_HOST)
+        pout = L.RaynFilmPlanes(ptr(outs, "color"), None, ptr(outs, "background"), None, L.MEM_HOST)
+        desc = denoise_desc(iterations, sigma_color, sigma_normal, sigma_alpha)
+        L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
+        return {k: v.reshape(np.shape(planes[k])) for k, v in outs.items()}
 
     # ---- known-answer entry points (tests) ----
     def kat_detmath(self, op, a, b=None):
@@ -284,6 +314,17 @@ class Film:
             Image.fromarray(px[:, :, 0] if pil == "L" else px, pil).save(path)
             written.append(path)
         return written
+
+    def denoise(self, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
+        """Filters the Film's color and background channels in place (Renderer.denoise), guided by its normal and alpha
+        channels.  Call it after render_frame_into and before save_to."""
+        for k in ("normal", "alpha"):
+            if k not in self.channels:
+                raise ValueError(f"Film.denoise needs the {k} channel")
+        if self._renderer is None:
+            self._renderer = Renderer(self._device)
+        w, h = self.res
+        self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha))
 
     def tonemapped_rgb8(self):
         """The display formula of save_to (film.rs:253-267): (color + background).saturated().gamma(2.2), y flipped."""

@@ -1,5 +1,5 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
-//   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--out file.ppm] [--dump planes.bin]
+//   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--denoise L] [--out file.ppm] [--dump planes.bin]
 // Renders one frame (frame 1, shutter 1/24 at 24 fps: main.rs:47-49,61-62), prints the reference's
 // "Done in {s} seconds." line (main.rs:79-82) and writes the display image with the formula of
 // Film::save_to (film.rs:253-267): (color + background).saturated().gamma_corrected(2.2), y flipped.
@@ -14,6 +14,8 @@ using namespace rayn;
 
 static constexpr float WORLD_RADIUS = 100.0f;    // setup.rs:33
 static constexpr int FRACTAL_ITERATIONS = 12;    // setup.rs:44
+// --denoise sigmas: the library's defaults (rayn_b200/film.py DENOISE_DEFAULTS, picked in DESIGN.md §4b)
+static constexpr float kDenoiseSigmaColor = 2.5f, kDenoiseSigmaNormal = 0.4f, kDenoiseSigmaAlpha = 0.5f;
 
 // setup.rs:46-169; `fractal` 0 = Mandelbox (the reference scene), 1 = authored Mandelbulb
 static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens) {
@@ -55,6 +57,7 @@ static CameraHandle setup_single_sphere(World& world, float rx, float ry) {  // 
 
 int main(int argc, char** argv) {
   int config = 3, W = 1280, H = 720, samples = 2, bounces = 3;  // setup.rs:16,22,30 defaults
+  int denoise = 0;  // a-trous levels run after the render, before --out / --dump; 0 = off
   bool res_set = false, samples_set = false, bounces_set = false;
   const char *out = nullptr, *dump = nullptr, *dump_scene = nullptr;
   for (int i = 1; i < argc; ++i) {
@@ -65,8 +68,13 @@ int main(int argc, char** argv) {
     else if (!strcmp(argv[i], "--out") && i + 1 < argc) out = argv[++i];
     else if (!strcmp(argv[i], "--dump") && i + 1 < argc) dump = argv[++i];
     else if (!strcmp(argv[i], "--dump-scene") && i + 1 < argc) dump_scene = argv[++i];
-    else { fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--out f.ppm] [--dump f.bin]\n"); return 2; }
+    else if (!strcmp(argv[i], "--denoise") && i + 1 < argc) denoise = atoi(argv[++i]);
+    else {
+      fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--denoise L] [--out f.ppm] [--dump f.bin]\n");
+      return 2;
+    }
   }
+  if (denoise < 0 || denoise > 8) { fprintf(stderr, "--denoise takes 1..8 levels (0 = off)\n"); return 2; }
   static const int cfg_res[6][2] = {{0, 0}, {256, 256}, {1024, 1024}, {1920, 1080}, {2048, 2048}, {7680, 4320}};
   static const int cfg_samples[6] = {0, 1, 32, 128, 64, 256}, cfg_bounces[6] = {0, 2, 4, 8, 4, 8};
   if (config < 1 || config > 5) { fprintf(stderr, "config must be 1..5\n"); return 2; }
@@ -101,6 +109,7 @@ int main(int argc, char** argv) {
     printf("Done in %.3f seconds.\n", secs);  // main.rs:79-82
     printf("%dx%d, %d spp, %d bounces: %.2f Msamples/s (device %.1f ms, %lld kernel launches)\n", W, H, 4 * samples, bounces,
            (double)film.stats.paths / secs / 1e6, film.stats.total_ms, (long long)film.stats.launches);
+    if (denoise) film.denoise(denoise, kDenoiseSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha);
     if (dump) {
       FILE* f = fopen(dump, "wb");
       if (!f) { perror(dump); return 1; }

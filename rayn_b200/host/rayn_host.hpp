@@ -274,6 +274,12 @@ class Film {
     rayn_b200_get_stats(ctx_, &stats);
     ++progressive_epoch;  // film.rs:657
   }
+  // Edge-avoiding a-trous filter of color and background in place, guided by normal and alpha (rayn_b200_film_denoise).
+  void denoise(int iterations, float sigma_color, float sigma_normal, float sigma_alpha) {
+    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    check(rayn_b200_film_denoise(ctx_, &d, w_, h_, &p, &p), ctx_);
+  }
   int width() const { return w_; }
   int height() const { return h_; }
   std::vector<float> color, alpha, background, normal;
