@@ -375,11 +375,65 @@ typedef struct RaynDenoiseDesc {
 int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* desc, int32_t width, int32_t height,
                                const RaynFilmPlanes* in, const RaynFilmPlanes* out);
 
+/* ---- progressive / adaptive rendering: a device film accumulator refined in sample rounds -----------------------
+ * Per-tile stopping rule after Dammertz, Hanika, Keller, Lensch (WSCG 2009; PAPERS.md): a tile's error compares the
+ * film of all its samples with the film of half of them (the rounds it rendered first, third, ...), weighted by
+ * 1/sqrt(I).  accum_create allocates all device state (13 floats per pixel, the round's 10 planes per pixel, per tile
+ * K, Kh, rounds, E), so render-pass sizing sees it.  Tile index = tile_x * n_tiles_y + tile_y on the grid of
+ * film.rs:399-404 (including its partial-tile quirk).
+ *
+ * accum_round(frame, desc): the ACTIVE tiles, chosen per tile before the round, are those with
+ *     rounds < max_rounds && (rounds < min_rounds || !(E <= threshold))
+ * They are rendered with `frame` (its tile_list / tile_offset / tile_stride are ignored) into the accumulator's own
+ * device planes m (already / spp), then folded in.  width, height and tile size must equal the accumulator's.
+ * A tile that stops never resumes, so all active tiles share one sample history: the CALLER passes tables for the
+ * samples they have not seen yet, i.e. rayn_b200_{host,device}_rd_tables_at with first_sample = the sum of spp of the
+ * earlier rounds (= `samples` of an active tile in accum_tiles).  The library cannot check this.  Active tiles whose
+ * round counts differ (a desc changed between rounds) are RAYN_ERR_INVALID_ARG.  Synchronous (the tile errors pick
+ * the next round's tiles).  *out_tiles_rendered (may be NULL) = active tiles; 0 = every tile has stopped, nothing ran.
+ * Exact statement, float unless marked, no contraction; n = (float)(4 * frame->samples); for every in-image pixel of
+ * an active tile:
+ *   S.x[c] = S.x[c] + m.x[c] * n          for color (3), alpha (1), background (3), normal (3)
+ *   if the tile's rounds is even before the round:  H[c] = H[c] + (m.color[c] + m.background[c]) * n
+ * per tile: K += 4*samples, Kh += 4*samples if H was updated (int64), rounds += 1.  A round that would take K past
+ * 2^24 is RAYN_ERR_INVALID_ARG (so (float)K is exact).  Then, for tiles with rounds >= 2, per pixel:
+ *   I[c] = (S.color[c] + S.background[c]) / (float)K,   A[c] = H[c] / (float)Kh
+ *   d = (|I0-A0| + |I1-A1|) + |I2-A2|,   s = (I0 + I1) + I2,   e = d / sqrtf(fmaxf(s, 0x1p-10f));  NaN e -> +inf
+ *   E = (double sum of (double)e over the tile's in-image pixels in ascending pixel index x + y*width, strictly
+ *        sequential) / (double)count
+ * Tiles with fewer than 2 rounds have E = +inf.  A negative threshold never stops a tile (E is never negative):
+ * uniform progressive rendering.
+ * accum_resolve: out.x[c] = S.x[c] / (float)K of the pixel's tile; pixels outside the tile grid are 0.  After one round
+ * of power-of-two spp this is render_frame's film bit for bit.  Planes are host or device (out->space), any may be
+ * NULL; synchronous.  RAYN_ERR_INVALID_ARG before the first round.
+ * accum_tiles: host arrays of n_tiles_x * n_tiles_y entries (either may be NULL): E and samples (= K) per tile.   */
+typedef struct RaynAccum RaynAccum;
+typedef struct RaynAdaptiveDesc {
+  int32_t min_rounds; /* >= 2: every tile gets at least this many rounds                            */
+  int32_t max_rounds; /* >= min_rounds: no tile gets more                                           */
+  float threshold;    /* not NaN: a tile stops once its error E <= threshold; < 0 = never (uniform)  */
+} RaynAdaptiveDesc;
+int32_t rayn_b200_accum_create(RaynContext* ctx, int32_t width, int32_t height, int32_t tile_w, int32_t tile_h,
+                               RaynAccum** out);
+void rayn_b200_accum_destroy(RaynAccum* acc);
+int32_t rayn_b200_accum_round(RaynContext* ctx, RaynAccum* acc, const RaynFrameDesc* frame,
+                              const RaynAdaptiveDesc* desc, int32_t* out_tiles_rendered);
+int32_t rayn_b200_accum_tiles(RaynContext* ctx, const RaynAccum* acc, double* err, int64_t* samples);
+int32_t rayn_b200_accum_resolve(RaynContext* ctx, const RaynAccum* acc, const RaynFilmPlanes* out);
+
 /* ---- host-side input builders (pure CPU; stand in for crates the Rust host owns) ----
  * quasi-rd R_d tables (sampler.rs:18-37), rand SmallRng scramble (film.rs:460-461),
  * FilterImportanceSampler::new(BlackmanHarris) (filter.rs:13-49,196-218).               */
 int32_t rayn_b200_host_rd_tables(int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,
                                  float* out_1d, float* out_2d);
+/* samples [first_sample, first_sample + spp) of the same sequences: element n of set i is the R_d value at index
+ * ((offset + i) << 32) + first_sample + n + 1 (2D sets offset by sets_1d, as above); rd_tables is first_sample = 0.
+ * first_sample + spp > 2^32 is RAYN_ERR_INVALID_ARG.  For sample rounds of one film (rayn_b200_accum_round).       */
+int32_t rayn_b200_host_rd_tables_at(int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset, uint64_t first_sample,
+                                    float* out_1d, float* out_2d);
+/* the same in device memory (DEVICE pointers, bit-identical to the host builder), synchronous */
+int32_t rayn_b200_device_rd_tables_at(RaynContext* ctx, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,
+                                      uint64_t first_sample, float* out_1d_dev, float* out_2d_dev);
 int32_t rayn_b200_host_scramble(int32_t width, int32_t height, float* out);
 int32_t rayn_b200_host_fis_blackman_harris(float radius, float* out512);
 /* the same tables / scramble plane generated directly in device memory (DEVICE pointers; bit-identical

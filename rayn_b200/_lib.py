@@ -103,6 +103,10 @@ class RaynDenoiseDesc(C.Structure):
     _fields_ = [("iterations", i32), ("sigma_color", f32), ("sigma_normal", f32), ("sigma_alpha", f32)]
 
 
+class RaynAdaptiveDesc(C.Structure):
+    _fields_ = [("min_rounds", i32), ("max_rounds", i32), ("threshold", f32)]
+
+
 class RaynConfig(C.Structure):
     _fields_ = [("device", i32), ("max_paths_per_pass", i64), ("flags", i32)]
 
@@ -143,10 +147,17 @@ SYMBOLS = {
     "rayn_b200_film_unpack_tiles": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(i32), i32, C.c_void_p, C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_film_postprocess": (i32, [C.c_void_p, i32, i32, i32, C.POINTER(RaynFilmPlanes), C.c_void_p, i32]),
     "rayn_b200_film_denoise": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_accum_create": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(C.c_void_p)]),
+    "rayn_b200_accum_destroy": (None, [C.c_void_p]),
+    "rayn_b200_accum_round": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynAdaptiveDesc), C.POINTER(i32)]),
+    "rayn_b200_accum_tiles": (i32, [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.POINTER(i64)]),
+    "rayn_b200_accum_resolve": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_host_rd_tables": (i32, [i32, i32, i32, C.c_uint64, fp, fp]),
+    "rayn_b200_host_rd_tables_at": (i32, [i32, i32, i32, C.c_uint64, C.c_uint64, fp, fp]),
     "rayn_b200_host_scramble": (i32, [i32, i32, fp]),
     "rayn_b200_host_fis_blackman_harris": (i32, [f32, fp]),
     "rayn_b200_device_frame_inputs": (i32, [C.c_void_p, i32, i32, i32, i32, i32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rayn_b200_device_rd_tables_at": (i32, [C.c_void_p, i32, i32, i32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
     "rayn_b200_host_tile_grid": (i32, [i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]),
     "rayn_b200_kat_detmath": (i32, [C.c_void_p, i32, i64, fp, fp, fp]),
     "rayn_b200_kat_sdf_dist": (i32, [C.c_void_p, C.POINTER(RaynHitable), i64, fp, fp]),
@@ -161,7 +172,7 @@ SYMBOLS = {
     "rayn_b200_debug_read_queue_log": (i64, [C.c_void_p, C.POINTER(i32), i64]),
 }
 
-HOST_SYMBOLS = ("rayn_b200_host_rd_tables", "rayn_b200_host_scramble", "rayn_b200_host_fis_blackman_harris", "rayn_b200_host_tile_grid")
+HOST_SYMBOLS = ("rayn_b200_host_rd_tables", "rayn_b200_host_rd_tables_at", "rayn_b200_host_scramble", "rayn_b200_host_fis_blackman_harris", "rayn_b200_host_tile_grid")
 
 _lib = None
 _hostlib = None

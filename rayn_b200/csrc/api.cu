@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "rt_accum.cuh"
 #include "rt_denoise.cuh"
 #include "rt_kernels.cuh"
 #ifdef RAYN_LEGACY_KERNELS
@@ -1289,10 +1290,167 @@ int32_t rayn_b200_device_frame_inputs(RaynContext* ctx, int32_t W, int32_t H, in
   CU(cudaSetDevice(ctx->device));
   CU(cudaDeviceSynchronize());
   const long long n = (long long)spp * (sets_1d + sets_2d);
-  if (n > 0) k_gen_rd_tables<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(spp, sets_1d, sets_2d, offset, s1, s2);
+  if (n > 0) k_gen_rd_tables<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(spp, sets_1d, sets_2d, offset, 0ull, s1, s2);
   if (scramble) k_gen_scramble<<<(unsigned)(((long long)W * H + 255) / 256), 256, 0, ctx->stream>>>(W, H, scramble);
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream));
+  return RAYN_OK;
+}
+
+int32_t rayn_b200_device_rd_tables_at(RaynContext* ctx, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset, uint64_t first,
+                                      float* s1, float* s2) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (spp <= 0 || sets_1d < 0 || sets_2d < 0 || (sets_1d && !s1) || (sets_2d && !s2))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "device_rd_tables_at: bad argument");
+  if (first > (1ull << 32) - (uint64_t)spp)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "device_rd_tables_at: first_sample + spp = %llu exceeds 2^32", (unsigned long long)first + spp);
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaDeviceSynchronize());
+  const long long n = (long long)spp * (sets_1d + sets_2d);
+  if (n > 0) k_gen_rd_tables<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(spp, sets_1d, sets_2d, offset, first, s1, s2);
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(ctx->stream));
+  return RAYN_OK;
+}
+
+// ---- film accumulator (rt_accum.cuh; statement in include/rayn_b200.h) ----------------------------------------------
+struct RaynAccum {
+  int device = 0, W = 0, H = 0, tw = 0, th = 0, ntx = 0, nty = 0, n_tiles = 0;
+  int64_t rounds_run = 0;     // rounds that rendered at least one tile
+  float* state = nullptr;     // S and H, 13 floats per pixel (rt_accum.cuh)
+  float* planes = nullptr;    // the round's render (and resolve staging for host planes), 10 floats per pixel
+  void* tile_mem = nullptr;   // AccumTiles arrays + the round's tile list
+  AccumTiles dt{};
+  int* d_list = nullptr;
+  // host copies of the per-tile state, refreshed after every round
+  std::vector<double> E;
+  std::vector<long long> K, Kh;
+  std::vector<int> rounds;
+};
+
+static void accum_free(RaynAccum* a) {
+  cudaFree(a->state), cudaFree(a->planes), cudaFree(a->tile_mem);
+  delete a;
+}
+
+int32_t rayn_b200_accum_create(RaynContext* ctx, int32_t W, int32_t H, int32_t tw, int32_t th, RaynAccum** out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!out || W <= 0 || H <= 0 || tw <= 0 || th <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_create: bad argument");
+  *out = nullptr;
+  CU(cudaSetDevice(ctx->device));
+  RaynAccum* a = new RaynAccum();
+  a->device = ctx->device, a->W = W, a->H = H, a->tw = tw, a->th = th;
+  tile_grid_of(W, H, tw, th, &a->ntx, &a->nty);
+  const int nt = a->n_tiles = a->ntx * a->nty;
+  const size_t npx = (size_t)W * H;
+  const size_t tile_bytes = (size_t)nt * (sizeof(double) + 2 * sizeof(long long) + 2 * sizeof(int));
+  cudaError_t e = cudaMalloc((void**)&a->state, npx * 13 * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc((void**)&a->planes, npx * 10 * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&a->tile_mem, tile_bytes);
+  a->E.assign(nt, INFINITY), a->K.assign(nt, 0), a->Kh.assign(nt, 0), a->rounds.assign(nt, 0);
+  if (e == cudaSuccess) {
+    char* p = (char*)a->tile_mem;
+    a->dt.E = (double*)p, a->dt.K = (long long*)(p + nt * sizeof(double)), a->dt.Kh = a->dt.K + nt;
+    a->dt.rounds = (int*)(a->dt.Kh + nt), a->d_list = a->dt.rounds + nt;
+    e = cudaMemsetAsync(a->state, 0, npx * 13 * sizeof(float), ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->dt.K, 0, (size_t)nt * (2 * sizeof(long long) + sizeof(int)), ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a->dt.E, a->E.data(), nt * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  }
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    accum_free(a);
+    return fail(ctx, e == cudaErrorMemoryAllocation ? RAYN_ERR_OOM : RAYN_ERR_CUDA, "accum_create (%dx%d): %s", W, H, cudaGetErrorString(e));
+  }
+  *out = a;
+  return RAYN_OK;
+}
+
+void rayn_b200_accum_destroy(RaynAccum* a) {
+  if (!a) return;
+  cudaSetDevice(a->device);
+  cudaDeviceSynchronize();
+  accum_free(a);
+}
+
+int32_t rayn_b200_accum_round(RaynContext* ctx, RaynAccum* a, const RaynFrameDesc* f, const RaynAdaptiveDesc* d, int32_t* out_tiles) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (out_tiles) *out_tiles = 0;
+  if (!a || !f || !d) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: NULL argument");
+  if (a->device != ctx->device) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: the accumulator lives on device %d, the context on %d", a->device, ctx->device);
+  if (d->min_rounds < 2 || d->max_rounds < d->min_rounds || d->threshold != d->threshold)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: need 2 <= min_rounds (%d) <= max_rounds (%d) and a threshold that is not NaN", d->min_rounds,
+                d->max_rounds);
+  if (f->width != a->W || f->height != a->H || f->tile_w != a->tw || f->tile_h != a->th)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: frame %dx%d tiles %dx%d, accumulator %dx%d tiles %dx%d", f->width, f->height, f->tile_w,
+                f->tile_h, a->W, a->H, a->tw, a->th);
+  if (f->samples <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: samples %d", f->samples);
+  std::vector<int> active;
+  for (int t = 0; t < a->n_tiles; ++t)
+    if (a->rounds[t] < d->max_rounds && (a->rounds[t] < d->min_rounds || !(a->E[t] <= (double)d->threshold))) active.push_back(t);
+  if (active.empty()) return RAYN_OK;
+  const long long n_int = 4ll * f->samples;
+  for (int t : active) {
+    if (a->rounds[t] != a->rounds[active[0]])
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: active tiles %d and %d have rendered %d and %d rounds; a stopped tile cannot resume", active[0], t,
+                  a->rounds[active[0]], a->rounds[t]);
+    if (a->K[t] + n_int > (1ll << 24))
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: tile %d would hold %lld samples per pixel, more than 2^24", t, a->K[t] + n_int);
+  }
+  RaynFilmPlanes dev{a->planes, a->planes + 3 * (size_t)a->W * a->H, a->planes + 4 * (size_t)a->W * a->H, a->planes + 7 * (size_t)a->W * a->H,
+                     RAYN_MEM_DEVICE};
+  int32_t rc = render_enqueue(ctx, f, &dev, &active, nullptr);
+  if (rc) return rc;
+  if ((rc = render_finish(ctx))) return rc;
+  cudaStream_t st = ctx->stream;
+  const int nt = a->n_tiles, na = (int)active.size();
+  CU(cudaMemcpyAsync(a->d_list, active.data(), na * sizeof(int), cudaMemcpyHostToDevice, st));
+  k_accum_fold<<<na, ACC_T, 0, st>>>(a->W, a->H, a->tw, a->th, a->nty, a->d_list, (float)n_int, n_int, a->planes, a->state, a->dt);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(a->E.data(), a->dt.E, nt * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(a->K.data(), a->dt.K, nt * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(a->Kh.data(), a->dt.Kh, nt * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(a->rounds.data(), a->dt.rounds, nt * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  a->rounds_run++;
+  if (out_tiles) *out_tiles = na;
+  return RAYN_OK;
+}
+
+int32_t rayn_b200_accum_tiles(RaynContext* ctx, const RaynAccum* a, double* err, int64_t* samples) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!a) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_tiles: accumulator is NULL");
+  if (err) std::copy(a->E.begin(), a->E.end(), err);
+  if (samples) std::copy(a->K.begin(), a->K.end(), samples);
+  return RAYN_OK;
+}
+
+int32_t rayn_b200_accum_resolve(RaynContext* ctx, const RaynAccum* a, const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!a || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_resolve: NULL argument");
+  if (out->space != RAYN_MEM_HOST && out->space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_resolve: bad memory space");
+  if (a->device != ctx->device) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_resolve: the accumulator lives on device %d, the context on %d", a->device, ctx->device);
+  if (a->rounds_run == 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_resolve: no round has been rendered");
+  if (!out->color && !out->alpha && !out->background && !out->normal) return RAYN_OK;
+  CU(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t npx = (size_t)a->W * a->H;
+  float *c = out->color, *al = out->alpha, *b = out->background, *n = out->normal;
+  if (out->space == RAYN_MEM_HOST) {  // resolve into the round's planes (free between rounds), then copy out
+    float* p = a->planes;
+    c = c ? p : nullptr, al = al ? p + 3 * npx : nullptr, b = b ? p + 4 * npx : nullptr, n = n ? p + 7 * npx : nullptr;
+  } else {
+    CU(cudaDeviceSynchronize());  // device planes may still be in use on another stream (e.g. torch's)
+  }
+  k_accum_resolve<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(a->W, a->H, a->tw, a->th, a->ntx, a->nty, a->state, a->dt.K, c, al, b, n);
+  CU(cudaGetLastError());
+  if (out->space == RAYN_MEM_HOST) {
+    if (c) CU(cudaMemcpyAsync(out->color, c, npx * 12, cudaMemcpyDeviceToHost, st));
+    if (al) CU(cudaMemcpyAsync(out->alpha, al, npx * 4, cudaMemcpyDeviceToHost, st));
+    if (b) CU(cudaMemcpyAsync(out->background, b, npx * 12, cudaMemcpyDeviceToHost, st));
+    if (n) CU(cudaMemcpyAsync(out->normal, n, npx * 12, cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
   return RAYN_OK;
 }
 

@@ -72,14 +72,20 @@ extern "C" {
 
 int32_t rayn_b200_host_rd_tables(int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset, float* out_1d,
                                  float* out_2d) {
-  if (spp <= 0 || sets_1d < 0 || sets_2d < 0 || (!out_1d && sets_1d) || (!out_2d && sets_2d))
+  return rayn_b200_host_rd_tables_at(spp, sets_1d, sets_2d, offset, 0, out_1d, out_2d);
+}
+
+// samples [first, first + spp) of every set: a later slice of the same sequence, for sample rounds of one film
+int32_t rayn_b200_host_rd_tables_at(int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset, uint64_t first, float* out_1d,
+                                    float* out_2d) {
+  if (spp <= 0 || sets_1d < 0 || sets_2d < 0 || (!out_1d && sets_1d) || (!out_2d && sets_2d) || first > (1ull << 32) - (uint64_t)spp)
     return RAYN_ERR_INVALID_ARG;
   for (int i = 0; i < sets_1d; ++i) {
-    uint64_t base = (offset + (uint64_t)i) << 32;
+    uint64_t base = ((offset + (uint64_t)i) << 32) + first;
     for (int n = 0; n < spp; ++n) out_1d[(size_t)spp * i + n] = rd_value(kAlpha1, base + (uint64_t)n + 1);
   }
   for (int i = 0; i < sets_2d; ++i) {
-    uint64_t base = (offset + (uint64_t)sets_1d + (uint64_t)i) << 32;
+    uint64_t base = ((offset + (uint64_t)sets_1d + (uint64_t)i) << 32) + first;
     for (int n = 0; n < spp; ++n) {
       out_2d[(size_t)2 * spp * i + 2 * n + 0] = rd_value(kAlpha2x, base + (uint64_t)n + 1);
       out_2d[(size_t)2 * spp * i + 2 * n + 1] = rd_value(kAlpha2y, base + (uint64_t)n + 1);

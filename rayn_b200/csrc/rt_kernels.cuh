@@ -1453,17 +1453,18 @@ RT_D float dev_rd_value(unsigned long long alpha, unsigned long long n) {
   const unsigned long long frac = alpha * n + 0x8000000000000000ull;
   return (float)(frac >> 40) * (1.0f / 16777216.0f);
 }
-__global__ void __launch_bounds__(256) k_gen_rd_tables(int spp, int sets_1d, int sets_2d, unsigned long long offset, float* __restrict__ s1,
-                                                       float* __restrict__ s2) {
+// samples [first, first + spp) of every set (first = 0: the frame's tables; later slices feed sample rounds)
+__global__ void __launch_bounds__(256) k_gen_rd_tables(int spp, int sets_1d, int sets_2d, unsigned long long offset, unsigned long long first,
+                                                       float* __restrict__ s1, float* __restrict__ s2) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long n1 = (long long)spp * sets_1d, n2 = (long long)spp * sets_2d;
   if (i < n1) {
     const int set = (int)(i / spp), n = (int)(i % spp);
-    s1[i] = dev_rd_value(0x9e3779b97f4a7c15ull, ((offset + (unsigned long long)set) << 32) + (unsigned long long)n + 1ull);
+    s1[i] = dev_rd_value(0x9e3779b97f4a7c15ull, ((offset + (unsigned long long)set) << 32) + first + (unsigned long long)n + 1ull);
   } else if (i < n1 + n2) {
     const long long j = i - n1;
     const int set = (int)(j / spp), n = (int)(j % spp);
-    const unsigned long long base = ((offset + (unsigned long long)sets_1d + (unsigned long long)set) << 32) + (unsigned long long)n + 1ull;
+    const unsigned long long base = ((offset + (unsigned long long)sets_1d + (unsigned long long)set) << 32) + first + (unsigned long long)n + 1ull;
     s2[2 * j + 0] = dev_rd_value(0xc13fa9a902a6328full, base);
     s2[2 * j + 1] = dev_rd_value(0x91e10da5c79e7b1cull, base);
   }

@@ -28,17 +28,19 @@ class FrameInputs:
     sampler.rs:18-37), per-pixel SmallRng scramble (film.rs:460-461) and the
     FilterImportanceSampler table (film.rs:429).  Built by the pure-CPU helpers of the C ABI."""
 
-    def __init__(self, width, height, samples, integrator, filt=None, frame=1):
+    def __init__(self, width, height, samples, integrator, filt=None, frame=1, first_sample=0):
         lib = L.host_lib()  # pure CPU: building frame inputs must not need (or map) the CUDA library
         filt = filt or BlackmanHarrisFilter(1.5)
         self.width, self.height, self.samples, self.spp, self.frame = width, height, samples, 4 * samples, frame
+        self.first_sample = first_sample  # > 0: samples [first_sample, first_sample + spp) of the frame, for a later sample round
         self.sets_1d = 1 + integrator.requested_1d_sample_sets()  # film.rs:431
         self.sets_2d = 2 + integrator.requested_2d_sample_sets()  # film.rs:432
         self.samples_1d = np.empty(self.spp * self.sets_1d, np.float32)
         self.samples_2d = np.empty(2 * self.spp * self.sets_2d, np.float32)
         self.scramble = np.empty(width * height, np.float32)
         self.fis = np.empty(L.RAYN_FIS_TABLE_SIZE, np.float32)
-        L.check(lib.rayn_b200_host_rd_tables(self.spp, self.sets_1d, self.sets_2d, frame, _fptr(self.samples_1d), _fptr(self.samples_2d)))
+        L.check(lib.rayn_b200_host_rd_tables_at(self.spp, self.sets_1d, self.sets_2d, frame, first_sample, _fptr(self.samples_1d),
+                                                _fptr(self.samples_2d)))
         L.check(lib.rayn_b200_host_scramble(width, height, _fptr(self.scramble)))
         L.check(lib.rayn_b200_host_fis_blackman_harris(filt.radius, _fptr(self.fis)))
 
@@ -79,10 +81,50 @@ def denoise_desc(iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=
     return L.RaynDenoiseDesc(int(iterations), s["sigma_color"], s["sigma_normal"], s["sigma_alpha"])
 
 
+# Adaptive sampling (Film.render_adaptive, rayn_b200_accum_round): a tile stops once its error E <= threshold.  Picked by
+# `tools/bench_adaptive.py` (DESIGN.md §4c): the largest speedup over uniform rounds at equal col+bg MSE on config 3
+# (1.12 at 0.025; thresholds of 0.04 and above lose to uniform rendering there).
+ADAPTIVE_THRESHOLD = 0.025
+ADAPTIVE_MAX_ROUNDS = 32
+
+
+def adaptive_desc(min_rounds=2, max_rounds=ADAPTIVE_MAX_ROUNDS, threshold=ADAPTIVE_THRESHOLD):
+    return L.RaynAdaptiveDesc(int(min_rounds), int(max_rounds), float(threshold))
+
+
 def tile_grid(width, height, tile_w, tile_h):
     nx, ny = C.c_int32(), C.c_int32()
     L.check(L.host_lib().rayn_b200_host_tile_grid(width, height, tile_w, tile_h, C.byref(nx), C.byref(ny)))
     return nx.value, ny.value
+
+
+class Accum:
+    """One device film accumulator (include/rayn_b200.h: rayn_b200_accum_*), made by Renderer.accum_create."""
+
+    def __init__(self, renderer, width, height, tile_size):
+        self._lib = renderer._lib
+        self.width, self.height = width, height
+        self.tile_size = tuple(tile_size)
+        self.n_tiles_x, self.n_tiles_y = tile_grid(width, height, *self.tile_size)
+        self.n_tiles = self.n_tiles_x * self.n_tiles_y
+        self._h = C.c_void_p()
+        L.check(self._lib.rayn_b200_accum_create(renderer.ctx, width, height, self.tile_size[0], self.tile_size[1], C.byref(self._h)),
+                renderer.ctx)
+
+    @property
+    def handle(self):
+        return self._h
+
+    def close(self):
+        if self._h:
+            self._lib.rayn_b200_accum_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class Renderer:
@@ -166,6 +208,38 @@ class Renderer:
         desc = denoise_desc(iterations, sigma_color, sigma_normal, sigma_alpha)
         L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
         return {k: v.reshape(np.shape(planes[k])) for k, v in outs.items()}
+
+    # ---- progressive / adaptive rendering (rayn_b200_accum_*) ----
+    def accum_create(self, width, height, tile_size):
+        return Accum(self, width, height, tile_size)
+
+    def accum_round(self, acc, frame_desc, min_rounds=2, max_rounds=ADAPTIVE_MAX_ROUNDS, threshold=ADAPTIVE_THRESHOLD):
+        """Renders the active tiles of `acc` with `frame_desc` and folds them in; returns how many tiles rendered (0: all
+        have stopped).  frame_desc's tables must hold the samples the active tiles have not seen: first_sample = their
+        `samples` in accum_tiles."""
+        d = adaptive_desc(min_rounds, max_rounds, threshold)
+        n = C.c_int32(0)
+        L.check(self._lib.rayn_b200_accum_round(self._ctx, acc.handle, C.byref(frame_desc), C.byref(d), C.byref(n)), self._ctx)
+        return n.value
+
+    def accum_tiles(self, acc):
+        """(E float64, samples per pixel int64) per tile, indexed by tile_x * n_tiles_y + tile_y."""
+        err, spp = np.empty(acc.n_tiles, np.float64), np.empty(acc.n_tiles, np.int64)
+        L.check(self._lib.rayn_b200_accum_tiles(self._ctx, acc.handle, err.ctypes.data_as(C.POINTER(C.c_double)),
+                                                spp.ctypes.data_as(C.POINTER(C.c_int64))), self._ctx)
+        return err, spp
+
+    def accum_resolve(self, acc, out=None):
+        """The accumulated film.  out=None: returns new host planes (dict, like render_host); else `out` is a RaynFilmPlanes
+        (host or device) written in place."""
+        planes = None
+        if out is None:
+            npx = acc.width * acc.height
+            planes = {k: np.zeros((1 if k == "alpha" else 3) * npx, np.float32) for k in CHANNELS}
+            out = L.RaynFilmPlanes(planes["color"].ctypes.data, planes["alpha"].ctypes.data, planes["background"].ctypes.data,
+                                   planes["normal"].ctypes.data, L.MEM_HOST)
+        L.check(self._lib.rayn_b200_accum_resolve(self._ctx, acc.handle, C.byref(out)), self._ctx)
+        return planes
 
     # ---- known-answer entry points (tests) ----
     def kat_detmath(self, op, a, b=None):
@@ -282,6 +356,61 @@ class Film:
         self.last_stats = self._renderer.stats()
         for k in self.channel_kinds:
             self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
+        self.progressive_epoch += 1  # film.rs:657
+
+    def render_adaptive(self, world, camera, integrator, filt, tile_size, frame, time_range, samples_per_round, min_rounds=2,
+                        max_rounds=ADAPTIVE_MAX_ROUNDS, threshold=ADAPTIVE_THRESHOLD, on_round=None):
+        """Progressive render in rounds of 4 * samples_per_round spp: every 16x16 (tile_size) tile keeps rendering until its
+        error E <= threshold (after at least min_rounds, at most max_rounds rounds; include/rayn_b200.h: accum_round).
+        A negative threshold renders every tile max_rounds times (uniform progressive rendering).  Fills self.channels
+        like render_frame_into and sets self.tile_errors / self.tile_samples (per tile index tile_x * n_tiles_y + tile_y).
+        on_round(film), if given, sees the film resolved after every round: a progressive preview.  Returns the number of
+        rounds rendered."""
+        import torch  # device buffers for the sample tables and the scramble plane
+        if self._renderer is None:
+            self._renderer = Renderer(self._device)
+        r, lib = self._renderer, self._renderer._lib
+        w, h = self.res
+        spp = 4 * samples_per_round
+        sets = (1 + integrator.requested_1d_sample_sets(), 2 + integrator.requested_2d_sample_sets())  # film.rs:431-432
+        r.upload_scene(world, camera)
+        dev = torch.device("cuda", r.device)
+        s1 = torch.empty(spp * sets[0], dtype=torch.float32, device=dev)
+        s2 = torch.empty(2 * spp * sets[1], dtype=torch.float32, device=dev)
+        scr = torch.empty(w * h, dtype=torch.float32, device=dev)
+        fis_h = np.empty(L.RAYN_FIS_TABLE_SIZE, np.float32)
+        L.check(L.host_lib().rayn_b200_host_fis_blackman_harris((filt or BlackmanHarrisFilter(1.5)).radius, _fptr(fis_h)))
+        fis = torch.from_numpy(fis_h).to(dev)
+        torch.cuda.synchronize(dev)
+        L.check(lib.rayn_b200_device_frame_inputs(r.ctx, w, h, spp, 0, 0, frame, None, None, scr.data_ptr()), r.ctx)
+        ptrs = (s1.data_ptr(), s2.data_ptr(), scr.data_ptr(), fis.data_ptr())
+        f = make_frame_desc(w, h, tile_size, samples_per_round, integrator, frame, time_range, ptrs, L.MEM_DEVICE, sets=sets)
+        acc = r.accum_create(w, h, tile_size)
+        rounds, first = 0, 0
+        try:
+            while True:
+                # every active tile has seen samples [0, first): this round renders the next spp of the same sequences
+                L.check(lib.rayn_b200_device_rd_tables_at(r.ctx, spp, sets[0], sets[1], frame, first, s1.data_ptr(), s2.data_ptr()), r.ctx)
+                if r.accum_round(acc, f, min_rounds, max_rounds, threshold) == 0:
+                    break
+                rounds += 1
+                first += spp
+                self.last_stats = r.stats()
+                if on_round is not None:
+                    self._take_accum(r, acc)
+                    on_round(self)
+            if on_round is None and rounds > 0:
+                self._take_accum(r, acc)
+        finally:
+            acc.close()
+        return rounds
+
+    def _take_accum(self, r, acc):
+        w, h = self.res
+        planes = r.accum_resolve(acc)
+        for k in self.channel_kinds:
+            self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
+        self.tile_errors, self.tile_samples = r.accum_tiles(acc)
         self.progressive_epoch += 1  # film.rs:657
 
     def save_to(self, write_channels, output_folder, base_name, transparent_background=False):

@@ -1,5 +1,6 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
-//   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--denoise L] [--out file.ppm] [--dump planes.bin]
+//   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] [--denoise L]
+//             [--out file.ppm] [--dump planes.bin]
 // Renders one frame (frame 1, shutter 1/24 at 24 fps: main.rs:47-49,61-62), prints the reference's
 // "Done in {s} seconds." line (main.rs:79-82) and writes the display image with the formula of
 // Film::save_to (film.rs:253-267): (color + background).saturated().gamma_corrected(2.2), y flipped.
@@ -16,6 +17,10 @@ static constexpr float WORLD_RADIUS = 100.0f;    // setup.rs:33
 static constexpr int FRACTAL_ITERATIONS = 12;    // setup.rs:44
 // --denoise sigmas: the library's defaults (rayn_b200/film.py DENOISE_DEFAULTS, picked in DESIGN.md §4b)
 static constexpr float kDenoiseSigmaColor = 2.5f, kDenoiseSigmaNormal = 0.4f, kDenoiseSigmaAlpha = 0.5f;
+
+// --adaptive: the library's defaults (rayn_b200/film.py ADAPTIVE_THRESHOLD / ADAPTIVE_MAX_ROUNDS, picked in DESIGN.md §4c)
+static constexpr float kAdaptiveThreshold = 0.025f;
+static constexpr int kAdaptiveMaxRounds = 32;
 
 // setup.rs:46-169; `fractal` 0 = Mandelbox (the reference scene), 1 = authored Mandelbulb
 static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens) {
@@ -58,6 +63,9 @@ static CameraHandle setup_single_sphere(World& world, float rx, float ry) {  // 
 int main(int argc, char** argv) {
   int config = 3, W = 1280, H = 720, samples = 2, bounces = 3;  // setup.rs:16,22,30 defaults
   int denoise = 0;  // a-trous levels run after the render, before --out / --dump; 0 = off
+  bool adaptive = false;  // --adaptive: rounds of --samples each until every tile's error <= threshold (at most --rounds)
+  float threshold = kAdaptiveThreshold;
+  int max_rounds = kAdaptiveMaxRounds;
   bool res_set = false, samples_set = false, bounces_set = false;
   const char *out = nullptr, *dump = nullptr, *dump_scene = nullptr;
   for (int i = 1; i < argc; ++i) {
@@ -69,12 +77,16 @@ int main(int argc, char** argv) {
     else if (!strcmp(argv[i], "--dump") && i + 1 < argc) dump = argv[++i];
     else if (!strcmp(argv[i], "--dump-scene") && i + 1 < argc) dump_scene = argv[++i];
     else if (!strcmp(argv[i], "--denoise") && i + 1 < argc) denoise = atoi(argv[++i]);
+    else if (!strcmp(argv[i], "--adaptive") && i + 1 < argc) adaptive = true, threshold = (float)atof(argv[++i]);
+    else if (!strcmp(argv[i], "--rounds") && i + 1 < argc) max_rounds = atoi(argv[++i]);
     else {
-      fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--denoise L] [--out f.ppm] [--dump f.bin]\n");
+      fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] "
+                      "[--denoise L] [--out f.ppm] [--dump f.bin]\n");
       return 2;
     }
   }
   if (denoise < 0 || denoise > 8) { fprintf(stderr, "--denoise takes 1..8 levels (0 = off)\n"); return 2; }
+  if (max_rounds < 2) { fprintf(stderr, "--rounds takes at least 2 rounds\n"); return 2; }
   static const int cfg_res[6][2] = {{0, 0}, {256, 256}, {1024, 1024}, {1920, 1080}, {2048, 2048}, {7680, 4320}};
   static const int cfg_samples[6] = {0, 1, 32, 128, 64, 256}, cfg_bounces[6] = {0, 2, 4, 8, 4, 8};
   if (config < 1 || config > 5) { fprintf(stderr, "config must be 1..5\n"); return 2; }
@@ -104,11 +116,21 @@ int main(int argc, char** argv) {
     const int frame = 1, frame_rate = 24;
     const float frame_start = (float)frame * (1.0f / (float)frame_rate), frame_end = frame_start + 1.0f / 24.0f;  // main.rs:61-62
     const auto t0 = std::chrono::steady_clock::now();
-    film.render_frame_into(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end, samples);
-    const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    printf("Done in %.3f seconds.\n", secs);  // main.rs:79-82
-    printf("%dx%d, %d spp, %d bounces: %.2f Msamples/s (device %.1f ms, %lld kernel launches)\n", W, H, 4 * samples, bounces,
-           (double)film.stats.paths / secs / 1e6, film.stats.total_ms, (long long)film.stats.launches);
+    if (adaptive) {
+      const int rounds = film.render_adaptive(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end, samples, 2, max_rounds, threshold);
+      const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      printf("Done in %.3f seconds.\n", secs);  // main.rs:79-82
+      int64_t total = 0, done = 0;
+      for (size_t t = 0; t < film.tile_samples.size(); ++t) total += film.tile_samples[t], done += film.tile_errors[t] <= (double)threshold;
+      printf("%dx%d, %d rounds of %d spp, %d bounces: %.1f spp per tile on average, %lld of %zu tiles below E = %g\n", W, H, rounds, 4 * samples,
+             bounces, (double)total / (double)std::max<size_t>(film.tile_samples.size(), 1), (long long)done, film.tile_samples.size(), threshold);
+    } else {
+      film.render_frame_into(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end, samples);
+      const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      printf("Done in %.3f seconds.\n", secs);  // main.rs:79-82
+      printf("%dx%d, %d spp, %d bounces: %.2f Msamples/s (device %.1f ms, %lld kernel launches)\n", W, H, 4 * samples, bounces,
+             (double)film.stats.paths / secs / 1e6, film.stats.total_ms, (long long)film.stats.launches);
+    }
     if (denoise) film.denoise(denoise, kDenoiseSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha);
     if (dump) {
       FILE* f = fopen(dump, "wb");

@@ -252,6 +252,71 @@ class Film {
     check(rayn_b200_host_rd_tables(spp, sets_1d, sets_2d, (uint64_t)frame, s1.data(), s2.data()), ctx_);  // film.rs:434
     check(rayn_b200_host_scramble(w_, h_, scr.data()), ctx_);                                              // film.rs:460-461
     check(rayn_b200_host_fis_blackman_harris(filter.radius, fis.data()), ctx_);                            // film.rs:429
+    upload_scene(world, camera);
+    RaynFrameDesc f = frame_desc(integrator, tile_w, tile_h, frame, t0, t1, samples, sets_1d, sets_2d);
+    f.samples_1d = s1.data(), f.samples_2d = s2.data(), f.scramble = scr.data(), f.fis_inverse_cdf = fis.data();
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    check(rayn_b200_render_frame(ctx_, &f, &p), ctx_);
+    rayn_b200_get_stats(ctx_, &stats);
+    ++progressive_epoch;  // film.rs:657
+  }
+  // Progressive render in rounds of 4*samples spp on a device film accumulator: every tile keeps rendering until its
+  // error E <= threshold, after at least min_rounds and at most max_rounds rounds (rayn_b200_accum_round).  Each round's
+  // tables are the next spp samples of the frame's sequences.  Leaves the film in the planes, the per-tile errors and
+  // samples in tile_errors / tile_samples; returns the number of rounds rendered.
+  int render_adaptive(const World& world, CameraHandle camera, const PathTracingIntegrator& integrator, const BlackmanHarrisFilter& filter,
+                      int tile_w, int tile_h, int frame, float t0, float t1, int samples, int min_rounds, int max_rounds, float threshold) {
+    const int spp = 4 * samples;
+    const int sets_1d = 1 + integrator.requested_1d_sample_sets(), sets_2d = 2 + integrator.requested_2d_sample_sets();
+    std::vector<float> s1((size_t)spp * sets_1d), s2((size_t)2 * spp * sets_2d), scr((size_t)w_ * h_), fis(RAYN_FIS_TABLE_SIZE);
+    check(rayn_b200_host_scramble(w_, h_, scr.data()), ctx_);
+    check(rayn_b200_host_fis_blackman_harris(filter.radius, fis.data()), ctx_);
+    upload_scene(world, camera);
+    RaynFrameDesc f = frame_desc(integrator, tile_w, tile_h, frame, t0, t1, samples, sets_1d, sets_2d);
+    f.samples_1d = s1.data(), f.samples_2d = s2.data(), f.scramble = scr.data(), f.fis_inverse_cdf = fis.data();
+    const RaynAdaptiveDesc d{min_rounds, max_rounds, threshold};
+    RaynAccum* acc = nullptr;
+    check(rayn_b200_accum_create(ctx_, w_, h_, tile_w, tile_h, &acc), ctx_);
+    int rounds = 0;
+    try {
+      for (uint64_t first = 0;; first += (uint64_t)spp) {
+        check(rayn_b200_host_rd_tables_at(spp, sets_1d, sets_2d, (uint64_t)frame, first, s1.data(), s2.data()), ctx_);
+        int32_t n = 0;
+        check(rayn_b200_accum_round(ctx_, acc, &f, &d, &n), ctx_);
+        if (n == 0) break;
+        ++rounds;
+        ++progressive_epoch;  // film.rs:657
+        rayn_b200_get_stats(ctx_, &stats);
+      }
+      RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+      check(rayn_b200_accum_resolve(ctx_, acc, &p), ctx_);
+      int ntx = 0, nty = 0;
+      check(rayn_b200_host_tile_grid(w_, h_, tile_w, tile_h, &ntx, &nty), ctx_);
+      tile_errors.assign((size_t)ntx * nty, 0.0), tile_samples.assign((size_t)ntx * nty, 0);
+      check(rayn_b200_accum_tiles(ctx_, acc, tile_errors.data(), tile_samples.data()), ctx_);
+    } catch (...) {
+      rayn_b200_accum_destroy(acc);
+      throw;
+    }
+    rayn_b200_accum_destroy(acc);
+    return rounds;
+  }
+  // Edge-avoiding a-trous filter of color and background in place, guided by normal and alpha (rayn_b200_film_denoise).
+  void denoise(int iterations, float sigma_color, float sigma_normal, float sigma_alpha) {
+    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    check(rayn_b200_film_denoise(ctx_, &d, w_, h_, &p, &p), ctx_);
+  }
+  int width() const { return w_; }
+  int height() const { return h_; }
+  std::vector<float> color, alpha, background, normal;
+  std::vector<double> tile_errors;    // render_adaptive: E per tile index tile_x * n_tiles_y + tile_y
+  std::vector<int64_t> tile_samples;  // ... and samples per pixel
+  RaynStats stats{};
+  int progressive_epoch = 0;
+
+ private:
+  void upload_scene(const World& world, CameraHandle camera) {
     std::vector<RaynLight> lights;
     for (const auto& l : world.lights) lights.push_back(l.pod);
     RaynSceneDesc sc{};
@@ -263,30 +328,16 @@ class Film {
                            world.volume_params.coeff_extinction};
     sc.consts = world.consts;
     check(rayn_b200_upload_scene(ctx_, &sc), ctx_);
+  }
+  RaynFrameDesc frame_desc(const PathTracingIntegrator& integrator, int tile_w, int tile_h, int frame, float t0, float t1, int samples, int sets_1d,
+                           int sets_2d) const {
     RaynFrameDesc f{};
     f.width = w_, f.height = h_, f.tile_w = tile_w, f.tile_h = tile_h, f.samples = samples;
     f.max_bounces = integrator.max_bounces, f.volume_marches = integrator.volume_marches, f.frame = frame, f.t0 = t0, f.t1 = t1;
     f.sets_1d = sets_1d, f.sets_2d = sets_2d;
-    f.samples_1d = s1.data(), f.samples_2d = s2.data(), f.scramble = scr.data(), f.fis_inverse_cdf = fis.data();
     f.input_space = RAYN_MEM_HOST, f.tile_offset = 0, f.tile_stride = 1;
-    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
-    check(rayn_b200_render_frame(ctx_, &f, &p), ctx_);
-    rayn_b200_get_stats(ctx_, &stats);
-    ++progressive_epoch;  // film.rs:657
+    return f;
   }
-  // Edge-avoiding a-trous filter of color and background in place, guided by normal and alpha (rayn_b200_film_denoise).
-  void denoise(int iterations, float sigma_color, float sigma_normal, float sigma_alpha) {
-    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
-    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
-    check(rayn_b200_film_denoise(ctx_, &d, w_, h_, &p, &p), ctx_);
-  }
-  int width() const { return w_; }
-  int height() const { return h_; }
-  std::vector<float> color, alpha, background, normal;
-  RaynStats stats{};
-  int progressive_epoch = 0;
-
- private:
   int w_, h_;
   RaynContext* ctx_ = nullptr;
 };
