@@ -102,6 +102,31 @@ typedef struct RaynMaterial {
   float emission[3];   /* Emissive::new_splat                                              */
 } RaynMaterial;
 
+/* ---- Orbit-trap albedo: a per-hit albedo generator for SDF surfaces -----------------------------------------------
+ * rayn's Lambertian<AG> and Dielectric<AG, RG> take an `albedo_gen: WShadingParamGenerator<WSrgb>` evaluated per shading
+ * point (material.rs:75-83,91-115,150-192); RaynMaterial.albedo is its constant implementor.  This is the one other
+ * generator kind built here: an orbit-trap palette, the classic way of colouring fractal surfaces.  Exact statement, in
+ * float, no contraction:
+ *   point   p = fma3s(d, t, o) of the hit: the point whose normal get_shading_info estimates (sdf.rs:85-101)
+ *   trap    trap(h, p) starts at +inf and folds trap = (x < trap) ? x : trap (a NaN never replaces it), where x is
+ *     Mandelbox:  for each iteration MandelBox::dist runs at p, r2 = mag_sq of the box-folded point (ultraviolet dot with
+ *                 the build's mul_add: mul_add(x, x, mul_add(y, y, z * z))), before the min_rad_sq clamp (sdf.rs:181-187)
+ *     Mandelbulb: every m = dot(w, w) the estimator assigns: m = dot(p, p) at the start, then the m of each iteration it
+ *                 runs before bailout (iteration i runs while i < iterations && !(m > bailout^2))
+ *     iterations = 0 (either fractal): trap = +inf
+ *   palette s = !(trap > trap_lo) ? 0 : (trap >= trap_hi ? 1 : (trap - trap_lo) / (trap_hi - trap_lo));
+ *           a hit on an analytic sphere whose material has a trap has s = 1 (no orbit)
+ *   albedo  albedo[c] = albedo_lo[c] * (1 - s) + albedo_hi[c] * s, with (1 - s) computed once
+ * The albedo replaces RaynMaterial.albedo wherever that hit's BSDF reads it: the Lambertian f and scatter f, and the
+ * Dielectric diffuse term of f (next-event estimation) and of scatter.  Normals, offsets, sample dimensions, packet
+ * composition, light choice and the alpha / normal channels do not change; trap evaluations are not counted in
+ * RaynStats.sdf_evals_normals.                                                                                      */
+typedef struct RaynAlbedoTrap {
+  int32_t material;                 /* index into the uploaded scene's materials: LAMBERTIAN or DIELECTRIC, one entry per material */
+  float trap_lo, trap_hi;           /* finite, trap_lo < trap_hi                                                                   */
+  float albedo_lo[3], albedo_hi[3]; /* finite                                                                                      */
+} RaynAlbedoTrap;
+
 /* ---- Light (src/light.rs:5-17): SphereLight::new(pos, rad, emission) :27-34 -------- */
 typedef struct RaynLight {
   float pos[3];
@@ -277,6 +302,12 @@ const char* rayn_b200_last_error(const RaynContext* ctx); /* ctx may be NULL: gl
 
 /* World -> device.  Replaces the `&world` argument of film.rs:384.                      */
 int32_t rayn_b200_upload_scene(RaynContext* ctx, const RaynSceneDesc* scene);
+/* Replaces the orbit-trap list of the current scene (n = 0 clears it; traps may be NULL then).  upload_scene clears it,
+ * so a caller that never calls this renders exactly as before.  RAYN_ERR_NO_SCENE before an upload; RAYN_ERR_INVALID_ARG
+ * for a bad entry (material index out of range, Sky / Emissive material, duplicate material, n < 0 or
+ * > RAYN_MAX_MATERIALS, non-finite value, trap_lo >= trap_hi); the list is unchanged then.  Render calls with
+ * RAYN_FLAG_SIMPLE_MARCH (legacy test kernels) and a non-empty list return RAYN_ERR_UNSUPPORTED.                     */
+int32_t rayn_b200_set_albedo_traps(RaynContext* ctx, int32_t n, const RaynAlbedoTrap* traps);
 
 /* The drop-in for Film::render_frame_into (film.rs:382-628) + tile_finished (:660-691).
  * Host pointers: inputs are copied H2D and planes D2H inside the call.
@@ -458,6 +489,8 @@ int32_t rayn_b200_kat_sdf_dist(RaynContext* ctx, const RaynHitable* sdf, int64_t
  * 4, 5 = 1, 2 with the three-operation sphere-fold division (RAYN_ERR_INVALID_ARG unless its exhaustive check passes here) */
 int32_t rayn_b200_kat_sdf_dist2(RaynContext* ctx, const RaynHitable* sdf, int32_t variant, int64_t n,
                                 const float* points3, float* out);
+/* trap(sdf, p) per point (RaynAlbedoTrap above), through the device function k_normals evaluates */
+int32_t rayn_b200_kat_sdf_trap(RaynContext* ctx, const RaynHitable* sdf, int64_t n, const float* points3, float* out);
 /* Newton division of the Mandelbox sphere fold vs IEEE division: number of x among the n consecutive floats starting
  * at bit pattern first_bits for which num / x differs (must be 0 wherever the fast variants are selected)           */
 int32_t rayn_b200_kat_fastdiv(RaynContext* ctx, float num, uint32_t first_bits, int64_t n, int64_t* out_mismatches);

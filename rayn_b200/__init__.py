@@ -10,7 +10,7 @@ Package layout (only what the hot path needs):
   build.py   in-tree nvcc build of librayn_b200.so
 """
 from .scene import (BlackmanHarrisFilter, BoxFold, CameraStore, Dielectric, Emissive, HitableStore, Lambertian, Linear,  # noqa: F401
-                    MandelBox, Mandelbulb, MaterialStore, OrthographicCamera, PathTracingIntegrator, PinholeCamera,
+                    MandelBox, Mandelbulb, MaterialStore, OrbitTrapAlbedo, OrthographicCamera, PathTracingIntegrator, PinholeCamera,
                     RenderConsts, Sky, Sphere, SphereFold, SphereLight, Srgb, ThinLensCamera, TracedSDF, Vec3,
                     VolumeParams, World)
 from .film import Film, FrameInputs, Renderer  # noqa: F401

@@ -59,6 +59,10 @@ class RaynMaterial(C.Structure):
                 ("sky_bottom", f32 * 3), ("emission", f32 * 3)]
 
 
+class RaynAlbedoTrap(C.Structure):
+    _fields_ = [("material", i32), ("trap_lo", f32), ("trap_hi", f32), ("albedo_lo", f32 * 3), ("albedo_hi", f32 * 3)]
+
+
 class RaynLight(C.Structure):
     _fields_ = [("pos", f32 * 3), ("rad", f32), ("emission", f32 * 3)]
 
@@ -135,6 +139,8 @@ SYMBOLS = {
     "rayn_b200_film_gather": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_sync": (i32, [C.c_void_p]),
     "rayn_b200_kat_sdf_dist2": (i32, [C.c_void_p, C.POINTER(RaynHitable), i32, i64, fp, fp]),
+    "rayn_b200_set_albedo_traps": (i32, [C.c_void_p, i32, C.POINTER(RaynAlbedoTrap)]),
+    "rayn_b200_kat_sdf_trap": (i32, [C.c_void_p, C.POINTER(RaynHitable), i64, fp, fp]),
     "rayn_b200_kat_fastdiv": (i32, [C.c_void_p, f32, C.c_uint32, i64, C.POINTER(i64)]),
     "rayn_b200_create": (i32, [C.POINTER(RaynConfig), C.POINTER(C.c_void_p)]),
     "rayn_b200_destroy": (None, [C.c_void_p]),

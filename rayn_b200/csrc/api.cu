@@ -67,6 +67,7 @@ struct RaynContext {
   // pass buffers
   int64_t alloc_paths = 0, alloc_q = 0, alloc_seg = 0;
   int alloc_lc_ns = 0;
+  bool alloc_trap = false;  // PassBufs::trap_s is allocated
   int alloc_tiles = 0;
   int64_t alloc_segcnt = 0;  // ints in PassBufs::seg_cnt
   size_t pass_bytes = 0;
@@ -75,8 +76,9 @@ struct RaynContext {
   int* d_batch_prefix = nullptr;  // [alloc_tiles + 1]
   int* d_work_ctr = nullptr;      // [WC_TOTAL] global work counters of the persistent kernels
   int n_sm = 148;
-  int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT];  // occ_ext[constant threshold][variant]
+  int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT], occ_nrm_trap[SDFV_COUNT];  // occ_ext[constant threshold][variant]
   int occ_pre = 8, occ_post = 8, occ_sph = 8;  // resident CTAs per SM of the work-list kernels
+  int occ_pre_trap = 8, occ_post_trap = 8;     // ... of the shading kernels of scenes with orbit-trap albedos
   int sdf_var[RAYN_MAX_HITABLES];  // march-kernel variant of every SDF hitable of the uploaded scene (rt_sdf2.cuh::sdf_variant)
   struct Div3Check { float min_r2, fixed_r2; bool ok; };
   std::vector<Div3Check> div3_cache;  // exhaustive fastdiv2_3 checks already run on this device
@@ -161,29 +163,32 @@ static void free_pass(RaynContext* c) {
   cudaFree(c->d_batch_prefix);
   c->d_batch_prefix = nullptr;
   cudaFree(p.nrm), cudaFree(p.vis), cudaFree(p.seg_a), cudaFree(p.seg_b), cudaFree(p.lc_c), cudaFree(p.lc_t), cudaFree(p.seg_cnt), cudaFree(p.slot_prefix);
+  cudaFree(p.trap_s);
   unsigned long long* counters = p.counters;
   memset(&p, 0, sizeof p);
   p.counters = counters;
   c->d_tile_ids = nullptr;
   c->alloc_paths = c->alloc_q = c->alloc_seg = 0;
   c->alloc_lc_ns = 0;
+  c->alloc_trap = false;
   c->alloc_tiles = 0;
   c->alloc_segcnt = 0;
   c->pass_bytes = 0;
 }
 
 // bytes of pass state per path (what ensure_pass allocates), used to size passes against free device memory
-static size_t pass_bytes_per_path(int R, int QS, int seg_per_path, int lc_ns) {
+static size_t pass_bytes_per_path(int R, int QS, int seg_per_path, int lc_ns, bool trap) {
   return 6 * sizeof(float4) + 2 * sizeof(uint32_t) + 2 * sizeof(int) + (size_t)(((double)QS / R) * sizeof(int) + 1) + (size_t)lc_ns * sizeof(float4) +
-         (lc_ns > 4 ? 8 * sizeof(float) : 0) + (size_t)seg_per_path * 2 * sizeof(float4);
+         (lc_ns > 4 ? 8 * sizeof(float) : 0) + (size_t)seg_per_path * 2 * sizeof(float4) + (trap ? sizeof(float) : 0);
 }
 
-static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg_per_path_total, int n_sdf, int lc_ns) {
+// trap: the scene has orbit-trap albedos, so the per-path palette coordinate PassBufs::trap_s is needed as well
+static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg_per_path_total, int n_sdf, int lc_ns, bool trap) {
   const int64_t need_paths = (int64_t)n_tiles * R, need_q = (int64_t)n_tiles * QS;
   const int64_t need_seg = need_paths * seg_per_path_total;  // all SDF queues together
   const int64_t need_segcnt = (int64_t)n_tiles * ((QS + SEG_SLOTS - 1) / SEG_SLOTS) * RAYN_MAX_HITABLES;
   if (need_paths <= ctx->alloc_paths && need_q <= ctx->alloc_q && n_tiles <= ctx->alloc_tiles && need_seg <= ctx->alloc_seg && lc_ns <= ctx->alloc_lc_ns &&
-      need_segcnt <= ctx->alloc_segcnt)
+      need_segcnt <= ctx->alloc_segcnt && (!trap || ctx->alloc_trap))
     return RAYN_OK;
   free_pass(ctx);
   PassBufs& p = ctx->pb;
@@ -228,7 +233,9 @@ static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg
     PASS_ALLOC(p.lc_c, need_paths * lc_ns * sizeof(float4));
     if (lc_ns > 4) PASS_ALLOC(p.lc_t, need_paths * 8 * sizeof(float));
   }
+  if (trap) PASS_ALLOC(p.trap_s, need_paths * sizeof(float));
 #undef PASS_ALLOC
+  ctx->alloc_trap = trap;
   ctx->alloc_lc_ns = lc_ns;
   ctx->alloc_paths = need_paths;
   ctx->alloc_q = need_q;
@@ -350,10 +357,13 @@ int32_t rayn_b200_create(const RaynConfig* cfg, RaynContext** out_ctx) {
     DISPATCH_SDFV(v, e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[0][v], k_extend_march<V, false>, EXT_T, 0);
                   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[1][v], k_extend_march<V, true>, EXT_T, 0);
                   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_shd[v], k_shadow<V>, SHD_T, 0);
-                  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_nrm[v], k_normals<V>, SLOT_BLOCK, 0));
+                  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_nrm[v], k_normals<V, false>, SLOT_BLOCK, 0);
+                  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_nrm_trap[v], k_normals<V, true>, SLOT_BLOCK, 0));
   }
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre, k_shade_pre, SLOT_BLOCK, 0);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post, k_shade_post, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre, k_shade_pre<false>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post, k_shade_post<false>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre_trap, k_shade_pre<true>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post_trap, k_shade_post<true>, SLOT_BLOCK, 0);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_sph, k_extend_spheres, EXT_BATCH, 0);
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -482,7 +492,36 @@ int32_t rayn_b200_upload_scene(RaynContext* ctx, const RaynSceneDesc* s) {
   }
   for (int i = 0; i < d.n_hit; ++i)
     ctx->sdf_var[i] = d.hit[i].kind == RAYN_HITABLE_SPHERE ? -1 : sdf_variant(d.hit[i], !(ctx->flags & RAYN_FLAG_NO_DIV3) && div3_verified(ctx, d.hit[i]));
-  ctx->has_scene = true;
+  ctx->has_scene = true;  // the memset above cleared the orbit-trap list (trap_mask = 0)
+  return RAYN_OK;
+}
+
+int32_t rayn_b200_set_albedo_traps(RaynContext* ctx, int32_t n, const RaynAlbedoTrap* traps) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "set_albedo_traps before upload_scene");
+  if (n < 0 || n > RAYN_MAX_MATERIALS) return fail(ctx, RAYN_ERR_INVALID_ARG, "n = %d traps not in [0,%d]", n, RAYN_MAX_MATERIALS);
+  if (n > 0 && !traps) return fail(ctx, RAYN_ERR_INVALID_ARG, "traps is NULL");
+  uint32_t mask = 0;
+  DevTrap tab[RAYN_MAX_MATERIALS];
+  memset(tab, 0, sizeof tab);
+  for (int i = 0; i < n; ++i) {
+    const RaynAlbedoTrap& t = traps[i];
+    const int m = t.material;
+    if (m < 0 || m >= ctx->scene.n_mat) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d out of range", i, m);
+    const int mk = ctx->scene.mat[m].kind;
+    if (mk != RAYN_MATERIAL_LAMBERTIAN && mk != RAYN_MATERIAL_DIELECTRIC)
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d is neither Lambertian nor Dielectric", i, m);
+    if (mask & (1u << m)) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d has a trap already", i, m);
+    bool finite = std::isfinite(t.trap_lo) && std::isfinite(t.trap_hi);
+    for (int c = 0; c < 3; ++c) finite = finite && std::isfinite(t.albedo_lo[c]) && std::isfinite(t.albedo_hi[c]);
+    if (!finite) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: non-finite value", i);
+    if (!(t.trap_lo < t.trap_hi)) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: trap_lo %g >= trap_hi %g", i, t.trap_lo, t.trap_hi);
+    mask |= 1u << m;
+    tab[m].lo = t.trap_lo, tab[m].hi = t.trap_hi;
+    for (int c = 0; c < 3; ++c) tab[m].a_lo[c] = t.albedo_lo[c], tab[m].a_hi[c] = t.albedo_hi[c];
+  }
+  ctx->scene.trap_mask = mask;
+  memcpy(ctx->scene.trap, tab, sizeof tab);
   return RAYN_OK;
 }
 
@@ -625,6 +664,8 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     motion |= ctx->scene.hit[i].kind == RAYN_HITABLE_SPHERE && (ctx->scene.hit[i].center_velocity[0] != 0.0f || ctx->scene.hit[i].center_velocity[1] != 0.0f ||
                                                                  ctx->scene.hit[i].center_velocity[2] != 0.0f);
   if (motion && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "time-varying sphere centres are not supported by the legacy test kernels");
+  const bool traps = ctx->scene.trap_mask != 0u;
+  if (traps && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "orbit-trap albedos are not supported by the legacy test kernels");
   // leading analytic spheres run inside raygen / shade_post (rt_kernels.cuh::fold_head); -1 = not folded (moving spheres need
   // the extend packet's lane-0 time; the legacy test kernels do the whole fold themselves)
   int fold_pre = -1;
@@ -645,7 +686,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   const int lc_ns = simple ? 0 : ns;                         // stored light contributions per path per depth
 
   // pass size: as many tiles as the requested path budget AND free device memory allow
-  const size_t bpp = pass_bytes_per_path(R, QS, seg_per_path, lc_ns);
+  const size_t bpp = pass_bytes_per_path(R, QS, seg_per_path, lc_ns, traps);
   size_t free_b = 0, total_b = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = (size_t)((double)(free_b + ctx->pass_bytes) * 0.90);
@@ -656,7 +697,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   tiles_per_pass = std::min(tiles_per_pass, 65535);
   tiles_per_pass = std::min<int>(tiles_per_pass, (int)std::max<size_t>(my_tiles.size(), 1));
   int32_t rc;
-  while ((rc = ensure_pass(ctx, tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns)) == RAYN_ERR_OOM && tiles_per_pass > 1)
+  while ((rc = ensure_pass(ctx, tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps)) == RAYN_ERR_OOM && tiles_per_pass > 1)
     tiles_per_pass = (tiles_per_pass + 1) / 2;  // fragmentation / another tenant: retry with half the pass
   if (rc) return rc;
   PassBufs pb = ctx->pb;
@@ -779,11 +820,17 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           if (!(mk == RAYN_MATERIAL_LAMBERTIAN || mk == RAYN_MATERIAL_DIELECTRIC || volume_on)) continue;
           const int v = ctx->sdf_var[sdf_idx[j]];
           timed_begin(ctx, RAYN_K_NORMALS);
-          DISPATCH_SDFV(v, (k_normals<V><<<resident(ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)));
+          if ((ctx->scene.trap_mask >> h.material) & 1u)  // the bin's material has an orbit-trap albedo: normals + trap
+            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
+          else
+            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
           timed_end(ctx, RAYN_K_NORMALS);
         }
         timed_begin(ctx, RAYN_K_SHADE_PRE);
-        k_shade_pre<<<resident(ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+        if (traps)
+          k_shade_pre<true><<<resident(ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+        else
+          k_shade_pre<false><<<resident(ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
         timed_end(ctx, RAYN_K_SHADE_PRE);
         if (ctx->scene.n_lights > 0) {
           for (int j = 0; j < n_sdf; ++j) {
@@ -794,7 +841,10 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           }
         }
         timed_begin(ctx, RAYN_K_SHADE_POST);
-        k_shade_post<<<resident(ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+        if (traps)
+          k_shade_post<true><<<resident(ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+        else
+          k_shade_post<false><<<resident(ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
         timed_end(ctx, RAYN_K_SHADE_POST);
       } else {
 #ifdef RAYN_LEGACY_KERNELS
@@ -1487,6 +1537,17 @@ int32_t rayn_b200_kat_sdf_dist(RaynContext* ctx, const RaynHitable* sdf, int64_t
   float* dout = tmp.up<float>(nullptr, n, &e);
   CU(e);
   k_kat_sdf_dist<<<blocks, 128, 0, ctx->stream>>>(*sdf, n, dp, dout);
+  KAT_EPILOGUE(out, dout, n, float)
+  return RAYN_OK;
+}
+int32_t rayn_b200_kat_sdf_trap(RaynContext* ctx, const RaynHitable* sdf, int64_t n, const float* points3, float* out) {
+  KAT_PROLOGUE
+  if (!sdf || !points3 || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_sdf_trap: NULL");
+  if (sdf->kind != RAYN_HITABLE_MANDELBOX && sdf->kind != RAYN_HITABLE_MANDELBULB) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_sdf_trap: not an SDF");
+  float* dp = tmp.up(points3, 3 * n, &e);
+  float* dout = tmp.up<float>(nullptr, n, &e);
+  CU(e);
+  k_kat_sdf_trap<<<blocks, 128, 0, ctx->stream>>>(*sdf, n, dp, dout);
   KAT_EPILOGUE(out, dout, n, float)
   return RAYN_OK;
 }

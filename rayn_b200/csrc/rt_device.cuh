@@ -105,6 +105,11 @@ RT_D float f_schlick(float cosv, float f0) { return f0 + (1.0f - f0) * dm::powi5
 // ------------------------------------------------------------------------------------------
 // Scene as a kernel-parameter block (constant bank: warp-uniform operands cost no load)
 // ------------------------------------------------------------------------------------------
+// orbit-trap palette of one material (RaynAlbedoTrap without its material index): 32 bytes
+struct DevTrap {
+  float lo, hi;
+  float a_lo[3], a_hi[3];
+};
 struct DevScene {
   int32_t n_hit, n_mat, n_lights;
   RaynHitable hit[RAYN_MAX_HITABLES];
@@ -115,11 +120,13 @@ struct DevScene {
   RaynRenderConsts rc;
   // derived at upload (api.cu::derive_scene_tables): the analytic spheres and the SDF hitables as compact lists in insertion
   // order, so that the shading kernels neither walk all hitables testing `kind` nor index 40-byte descriptors per lane
-  int32_t n_sph, n_sdf, sph_moving, pad_;
+  int32_t n_sph, n_sdf, sph_moving;
+  uint32_t trap_mask;                  // bit m: material m has an orbit-trap albedo (rayn_b200_set_albedo_traps); 0 = none
   int32_t sph_idx[RAYN_MAX_HITABLES];  // hitable index of sphere k
   int32_t sdf_idx[RAYN_MAX_HITABLES];  // hitable index of SDF ordinal j
   int32_t hit_ord[RAYN_MAX_HITABLES];  // hitable i is the hit_ord[i]-th sphere / SDF
   float4 sph[RAYN_MAX_HITABLES];       // centre.xyz, radius of sphere k (a moving sphere keeps its t = 0 centre here)
+  DevTrap trap[RAYN_MAX_MATERIALS];    // palette of material m where trap_mask bit m is set, zero elsewhere
 };
 
 // the `hit_threshold_at` closure of film.rs:540-551
@@ -164,7 +171,8 @@ RT_D bool eval_more(const SdfEval& e, const RaynHitable& h) {
   if (h.kind == RAYN_HITABLE_MANDELBULB) return e.it < h.iterations && !(e.m > h.bulb_bailout * h.bulb_bailout);
   return e.it < h.iterations;
 }
-RT_D void eval_step(SdfEval& e, const RaynHitable& h) {
+// r2_out (Mandelbox only, may be NULL): the squared radius the sphere fold divides by, before the min_rad_sq clamp
+RT_D void eval_step(SdfEval& e, const RaynHitable& h, float* r2_out = nullptr) {
   if (h.kind == RAYN_HITABLE_MANDELBULB) {
     const f3 w = e.w;
     const float m = e.m;
@@ -206,6 +214,7 @@ RT_D void eval_step(SdfEval& e, const RaynHitable& h) {
     p.y = dm::mul_add(cy, 2.0f, -p.y);
     p.z = dm::mul_add(cz, 2.0f, -p.z);
     const float r2 = mag_sq(p);
+    if (r2_out) *r2_out = r2;
     const float mul = dm::max(1.0f, h.fixed_rad_sq / dm::max(h.min_rad_sq, r2));
     p = p * mul;
     e.dr = e.dr * mul;
@@ -226,6 +235,34 @@ RT_D float sdf_dist(const RaynHitable& h, f3 p) {
   eval_start(e, h, p);
   while (eval_more(e, h)) eval_step(e, h);
   return eval_finish(e, h);
+}
+
+// Orbit trap of the distance estimator at p (include/rayn_b200.h, RaynAlbedoTrap): the min fold of the Mandelbox's r2 per
+// iteration, or of every m the Mandelbulb assigns.  One scalar run of the same state machine as sdf_dist.  The packed
+// Mandelbox variants of rt_sdf2.cuh differ from it only in how they divide AFTER r2 (the fast divisions equal IEEE division
+// for every divisor they can see), so every variant's iterations give the same r2 and the same trap as this one.
+RT_D float sdf_trap(const RaynHitable& h, f3 p) {
+  float trap = __int_as_float(0x7f800000);  // +inf
+  if (h.iterations <= 0) return trap;
+  SdfEval e;
+  eval_start(e, h, p);
+  const bool bulb = h.kind == RAYN_HITABLE_MANDELBULB;
+  if (bulb) trap = e.m < trap ? e.m : trap;
+  while (eval_more(e, h)) {
+    float r2 = 0.0f;
+    eval_step(e, h, &r2);
+    const float x = bulb ? e.m : r2;
+    trap = x < trap ? x : trap;
+  }
+  return trap;
+}
+// palette coordinate s of a trap value (include/rayn_b200.h)
+RT_D float trap_coord(const DevTrap& tp, float trap) {
+  return !(trap > tp.lo) ? 0.0f : (trap >= tp.hi ? 1.0f : (trap - tp.lo) / (tp.hi - tp.lo));
+}
+RT_D f3 trap_albedo(const DevTrap& tp, float s) {
+  const float r = 1.0f - s;
+  return {tp.a_lo[0] * r + tp.a_hi[0] * s, tp.a_lo[1] * r + tp.a_hi[1] * s, tp.a_lo[2] * r + tp.a_hi[2] * s};
 }
 
 // TracedSDF::hit per lane, sdf.rs:59-83 / SURVEY §9.1.  *evals counts dist() calls.
@@ -477,9 +514,9 @@ RT_D f3 bsdf_le(const RaynMaterial& m, f3 wo) {
   if (m.kind == RAYN_MATERIAL_EMISSIVE) return ld3(m.emission);  // :517-519
   return {0.0f, 0.0f, 0.0f};
 }
-// called as bsdf.f(wo, wi, n) (integrator.rs:230); see oracle note on argument naming.
-RT_D f3 bsdf_f(const RaynMaterial& m, f3 first, f3 second, f3 n) {
-  f3 albedo = ld3(m.albedo);
+// called as bsdf.f(wo, wi, n) (integrator.rs:230); see oracle note on argument naming.  `albedo` is what the material's
+// albedo generator gives at this hit: m.albedo, or an orbit-trap palette (trap_albedo).
+RT_D f3 bsdf_f(const RaynMaterial& m, f3 albedo, f3 first, f3 second, f3 n) {
   if (m.kind == RAYN_MATERIAL_LAMBERTIAN) return albedo / RT_PI;  // :139-141
   float rough = m.roughness;                                      // Dielectric :195-205
   float dotv = dm::max(0.0f, dot(first, n));
@@ -491,22 +528,22 @@ RT_D f3 bsdf_f(const RaynMaterial& m, f3 first, f3 second, f3 n) {
   f3 diffuse_f = albedo / RT_PI * (1.0f - fresnel);
   return spec_f + diffuse_f;
 }
+RT_D f3 bsdf_f(const RaynMaterial& m, f3 first, f3 second, f3 n) { return bsdf_f(m, ld3(m.albedo), first, second, n); }
 struct Scatter {
   f3 wi, f;
   float pdf;
 };
-RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 wo, const ShadingPoint& sp, float s1d, float u0, float u1, float u2,
+RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 albedo, f3 wo, const ShadingPoint& sp, float s1d, float u0, float u1, float u2,
                           float u3) {
   Scatter se;
   if (m.kind != RAYN_MATERIAL_DIELECTRIC) {  // Lambertian :118-137 (Emissive/Sky never scatter on the path)
     f3 ds = cosine_weighted(u0, u1);
     se.wi = normalized(mul(sp.basis, ds));
-    se.f = ld3(m.albedo) / RT_PI;
+    se.f = albedo / RT_PI;
     se.pdf = ds.z / RT_PI;
     return se;
   }
   // Dielectric :207-256
-  f3 albedo = ld3(m.albedo);
   float rough = m.roughness;
   f3 norm = sp.normal;
   float cosv = dm::abs(dot(norm, wo));
@@ -530,6 +567,9 @@ RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 wo, const ShadingPoint& sp, 
   se.f = fresnel_mask ? spec_f : diffuse_f;
   se.pdf = fresnel * spec_pdf + (1.0f - fresnel) * diffuse_pdf;
   return se;
+}
+RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 wo, const ShadingPoint& sp, float s1d, float u0, float u1, float u2, float u3) {
+  return bsdf_scatter(m, ld3(m.albedo), wo, sp, s1d, u0, u1, u2, u3);
 }
 
 RT_D int light_index(float s, int n_lights) {  // integrator.rs:76-77 (+ clamp, A10)

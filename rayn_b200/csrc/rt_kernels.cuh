@@ -73,6 +73,8 @@ struct PassBufs {
   // 128-slot blocks of the bin of SDF ordinal j; each row is an exclusive prefix over the tiles with the total at [n_tiles]
   int* slot_prefix;   // [(1 + RAYN_MAX_HITABLES) * prefix_stride]
   int prefix_stride;  // >= n_tiles + 1
+  float* trap_s;      // [paths] orbit-trap palette coordinate s of this depth's SDF hit, written by k_normals<V, true>; only
+                      // allocated when the scene has traps (DevScene::trap_mask != 0), NULL otherwise
 };
 
 enum { CNT_EXTEND_RAYS = 0, CNT_SHADE_LANES = 1, CNT_SHADOW_RAYS = 2, CNT_EVALS_EXTEND = 3, CNT_EVALS_SHADOW = 4,
@@ -634,8 +636,10 @@ __global__ void __launch_bounds__(EXT_T, MARCH_OCC(V)) k_extend_march(const __gr
 // K3b normals: TracedSDF::get_shading_info (sdf.rs:85-101) for the shading slots of SDF hitable `hk`:
 // sdfu's tetrahedral normals_fast (oracle/README.md A8) = 4 distance evaluations = 2 packed evaluations
 // per lane, specialised on the SDF like the march kernels.  Writes nrm[g] = (normal, offset_by).
+// TRAP (the hitable's material has an orbit-trap albedo): also one scalar trap evaluation at the same point, and
+// trap_s[g] = its palette coordinate s.  Bins without a trap run the TRAP = false kernel, which is the code they always ran.
 // ------------------------------------------------------------------------------------------
-template <int V>
+template <int V, bool TRAP>
 __global__ void __launch_bounds__(128, 8) k_normals(const __grid_constant__ DevScene sc, const PassBufs pb, const Thr thr, const int hk, const int j,
                                                     int* __restrict__ work_ctr) {
   const int* __restrict__ prefix = pb.slot_prefix + (size_t)(1 + j) * pb.prefix_stride;  // 128-slot blocks of this SDF's bins, all tiles
@@ -661,7 +665,8 @@ __global__ void __launch_bounds__(128, 8) k_normals(const __grid_constant__ DevS
       n = n + mk3(1.0f, 1.0f, 1.0f) * db.y;
       n = normalized(n);
       pb.nrm[g] = make_float4(n.x, n.y, n.z, eps);
-      evals += 4;
+      evals += 4;  // the trap evaluation is not counted (RaynStats.sdf_evals_normals stays 4 per SDF shading lane)
+      if (TRAP) pb.trap_s[g] = trap_coord(sc.trap[sc.hit[hk].material], sdf_trap(sc.hit[hk], point));
     }
   })
   warp_add(pb.counters + CNT_EVALS_NORMALS, evals);
@@ -680,8 +685,8 @@ struct LightContrib {
 };
 // round 0: surface_sample_one_light (integrator.rs:207-240) without the visibility factor;
 // round r>0: volume_sample_one_light (:242-281) for volume march r-1.
-RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, const ShadingPoint& sp, f3 wo, int round, float u0, float u1,
-                                float vol_sample, bool has_ext, float neg_rho_t) {
+RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, f3 albedo, const ShadingPoint& sp, f3 wo, int round, float u0,
+                                float u1, float vol_sample, bool has_ext, float neg_rho_t) {
   LightContrib r;
   f3 li;
   r.trans = 1.0f;
@@ -692,7 +697,7 @@ RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, con
     const float dist = mag(wi);
     wi = wi / dist;
     r.start = sp.point + sp.normal * dm::signum(dot(sp.normal, wi)) * sp.offset_by;
-    const f3 f = bsdf_f(mat, wo, wi, sp.normal) * dm::max(dot(sp.normal, wi), 0.0f);
+    const f3 f = bsdf_f(mat, albedo, wo, wi, sp.normal) * dm::max(dot(sp.normal, wi), 0.0f);
     const float tr = has_ext ? dm::exp(neg_rho_t * dist) : 1.0f;
     r.c = li * f * tr;
     r.den = pdf;
@@ -709,6 +714,15 @@ RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, con
     r.trans = has_ext ? dm::exp(neg_rho_t * vol_dist) : 1.0f;  // :122-126
   }
   return r;
+}
+
+// The albedo the hit's BSDF reads (include/rayn_b200.h, RaynAlbedoTrap): the material's constant, or its orbit-trap palette at
+// the s k_normals<V, true> stored for path g (s = 1 on an analytic sphere: no orbit).  trap_mask lives in the kernel-parameter
+// block, so the outer test is uniform.  Scenes without traps run the TRAP = false shading kernels, which never call this.
+RT_D f3 hit_albedo(const DevScene& sc, const PassBufs& pb, const RaynHitable& h, const RaynMaterial& mat, size_t g) {
+  if (sc.trap_mask != 0u && ((sc.trap_mask >> h.material) & 1u))
+    return trap_albedo(sc.trap[h.material], h.kind == RAYN_HITABLE_SPHERE ? 1.0f : pb.trap_s[g]);
+  return ld3(mat.albedo);
 }
 
 struct SlotCtx {  // what pre and post both derive for a shading slot
@@ -757,6 +771,7 @@ RT_D SlotCtx slot_ctx(const DevScene& sc, const DevFrame& fr, const PassBufs& pb
   return c;
 }
 
+template <bool TRAP>
 RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs& pb, const int depth, const Thr thr, const int ts, const int s) {
   const int nslots = pb.n_slots[ts];
   if ((s & ~31) >= nslots) return;  // warp-uniform
@@ -806,13 +821,14 @@ RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs&
         sp.offset_by = n4.w;
       }
       unsigned vis = 0xffffffffu;
+      const f3 tr_albedo = TRAP ? hit_albedo(sc, pb, h, mat, g) : mk3(0.0f, 0.0f, 0.0f);
       for (int round = (recv ? 0 : 1); round < n_rounds; ++round) {
         const unsigned wr = round == 0 ? cx.w0 : (round == 1 ? cx.w1 : cx.w2);
         const float vol_sample = round == 0 ? 0.0f : samp1(fr, cx.sample, cx.scramble, cx.set1 + 1);  // samples_1d[1], :115
 #pragma unroll 1
         for (int i = 0; i < 4; ++i) {
           const int set = round == 0 ? cx.set2 + i : cx.set2 + 4 + 4 * (round - 1) + i;
-          const LightContrib lc = light_contrib(sc.light[(wr >> (8 * i)) & 0xffu], mat, sp, wo, round, samp2(fr, 0, cx.sample, cx.scramble, set),
+          const LightContrib lc = light_contrib(sc.light[(wr >> (8 * i)) & 0xffu], mat, TRAP ? tr_albedo : ld3(mat.albedo), sp, wo, round, samp2(fr, 0, cx.sample, cx.scramble, set),
                                                 samp2(fr, 1, cx.sample, cx.scramble, set), vol_sample, has_ext, neg_rho_t);
           ++shadows;
           const int bit = round * 4 + i;
@@ -856,11 +872,21 @@ RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs&
 #ifndef RAYN_SHADE_PRE_OCC
 #define RAYN_SHADE_PRE_OCC 8  // resident CTAs per SM k_shade_pre is compiled for (tuning hook)
 #endif
+// TRAP: the scene has orbit-trap albedos (DevScene::trap_mask != 0); the TRAP = false kernel is the one scenes without traps run
+template <bool TRAP>
 __global__ void __launch_bounds__(128, RAYN_SHADE_PRE_OCC) k_shade_pre(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb,
                                                       const int depth, const Thr thr, int* __restrict__ work_ctr) {
   // row 0 of the work lists: the non-empty 128-slot blocks of every tile's shading queue
-  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_pre_slot(sc, fr, pb, depth, thr, ts, local * SLOT_BLOCK + threadIdx.x); })
+  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_pre_slot<TRAP>(sc, fr, pb, depth, thr, ts, local * SLOT_BLOCK + threadIdx.x); })
 }
+// k_shade_pre has the largest parameter list of the render kernels.  The scene limits of include/rayn_b200.h are sized for the
+// 4 KB kernel-parameter block; the orbit-trap palettes (DevScene::trap) leave little of it, so a later addition fails here.
+constexpr size_t param_align(size_t off, size_t a) { return (off + a - 1) / a * a; }
+constexpr size_t kShadePreParamBytes =
+    param_align(param_align(param_align(param_align(param_align(sizeof(DevScene), alignof(DevFrame)) + sizeof(DevFrame), alignof(PassBufs)) +
+                                            sizeof(PassBufs), alignof(int)) + sizeof(int), alignof(Thr)) + sizeof(Thr), alignof(int*)) +
+    sizeof(int*);
+static_assert(kShadePreParamBytes <= 4096, "k_shade_pre's parameters exceed the 4 KB the scene limits are sized for");
 
 // ------------------------------------------------------------------------------------------
 // K5 shadow sphere-march: TracedSDF::occluded per slot (sdf.rs:25-57, SURVEY §9.2) over the segment
@@ -969,6 +995,7 @@ __global__ void __launch_bounds__(SHD_T, MARCH_OCC(V)) k_shadow(const __grid_con
   if (V == SDFV_BULB) warp_add(pb.counters + CNT_BULB_ITERS_SHADOW, bulb_iters);
 }
 
+template <bool TRAP>
 RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs& pb, const int depth, const int pre_n, const int ts, const int s) {
   const int nslots = pb.n_slots[ts];
   if ((s & ~31) >= nslots) return;
@@ -1019,7 +1046,8 @@ RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs
   }
   if (recv) {  // :134-188
     const int setb = cx.set2 + 4 + 4 * fr.vm;
-    const Scatter se = bsdf_scatter(mat, wo, sp, samp1(fr, cx.sample, cx.scramble, cx.set1 + 3), samp2(fr, 0, cx.sample, cx.scramble, setb),
+    const Scatter se = bsdf_scatter(mat, TRAP ? hit_albedo(sc, pb, h, mat, g) : ld3(mat.albedo), wo, sp, samp1(fr, cx.sample, cx.scramble, cx.set1 + 3),
+                                    samp2(fr, 0, cx.sample, cx.scramble, setb),
                                     samp2(fr, 1, cx.sample, cx.scramble, setb), samp2(fr, 0, cx.sample, cx.scramble, setb + 1),
                                     samp2(fr, 1, cx.sample, cx.scramble, setb + 1));
     const float ndl = dm::abs(dot(se.wi, sp.normal));
@@ -1054,9 +1082,10 @@ RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs
   }
 }
 
+template <bool TRAP>
 __global__ void __launch_bounds__(128, 8) k_shade_post(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb,
                                                        const int depth, const int pre_n, int* __restrict__ work_ctr) {
-  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_post_slot(sc, fr, pb, depth, pre_n, ts, local * SLOT_BLOCK + threadIdx.x); })
+  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_post_slot<TRAP>(sc, fr, pb, depth, pre_n, ts, local * SLOT_BLOCK + threadIdx.x); })
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1549,6 +1578,11 @@ __global__ void __launch_bounds__(256) k_verify_div3(float num, unsigned first_b
            (__float_as_uint(fastdiv1_3(num, x)) != __float_as_uint(ref));
   }
   warp_add(mismatches, bad);
+}
+__global__ void k_kat_sdf_trap(const RaynHitable h, long long n, const float* p3, float* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  out[i] = sdf_trap(h, mk3(p3[3 * i], p3[3 * i + 1], p3[3 * i + 2]));  // the function k_normals<V, true> calls
 }
 __global__ void k_kat_sdf_hit(const RaynHitable h, const RaynRenderConsts rc, long long n, const float* o3, const float* d3,
                               const float* t_max, Thr thr, float* out) {

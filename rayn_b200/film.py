@@ -154,9 +154,19 @@ class Renderer:
         return self._ctx
 
     def upload_scene(self, world, camera):
+        """Uploads the scene, then its orbit-trap albedos (OrbitTrapAlbedo materials), if it has any."""
         desc, keep = world.flatten(camera)
         self._keep = (desc, keep)
         L.check(self._lib.rayn_b200_upload_scene(self._ctx, C.byref(desc)), self._ctx)
+        traps = world.albedo_traps()
+        if traps:
+            self.set_albedo_traps(traps)
+
+    def set_albedo_traps(self, traps):
+        """Replaces the orbit-trap list of the uploaded scene (include/rayn_b200.h: rayn_b200_set_albedo_traps): a list of
+        RaynAlbedoTrap, e.g. World.albedo_traps(); [] clears it."""
+        arr = (L.RaynAlbedoTrap * max(len(traps), 1))(*traps)
+        L.check(self._lib.rayn_b200_set_albedo_traps(self._ctx, len(traps), arr), self._ctx)
 
     def upload_scene_desc(self, desc):
         L.check(self._lib.rayn_b200_upload_scene(self._ctx, C.byref(desc)), self._ctx)
@@ -259,6 +269,13 @@ class Renderer:
         p = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
         out = np.empty(len(p), np.float32)
         L.check(self._lib.rayn_b200_kat_sdf_dist2(self._ctx, C.byref(hitable), variant, len(p), _fptr(p), _fptr(out)), self._ctx)
+        return out
+
+    def kat_sdf_trap(self, hitable, points):
+        """orbit trap per point on the device (the function k_normals evaluates for trap materials)"""
+        p = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+        out = np.empty(len(p), np.float32)
+        L.check(self._lib.rayn_b200_kat_sdf_trap(self._ctx, C.byref(hitable), len(p), _fptr(p), _fptr(out)), self._ctx)
         return out
 
     def kat_fastdiv(self, num, first_bits, n):

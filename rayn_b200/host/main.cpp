@@ -1,6 +1,8 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
 //   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] [--denoise L]
-//             [--out file.ppm] [--dump planes.bin]
+//             [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out file.ppm] [--dump planes.bin]
+// --orbit-trap colours the fractal of configs 2-5 by orbit trap: albedo (R0 G0 B0) at trap LO, (R1 G1 B1) at HI
+// (include/rayn_b200.h, RaynAlbedoTrap; tools/trap_range.py prints a range for config 3).
 // Renders one frame (frame 1, shutter 1/24 at 24 fps: main.rs:47-49,61-62), prints the reference's
 // "Done in {s} seconds." line (main.rs:79-82) and writes the display image with the formula of
 // Film::save_to (film.rs:253-267): (color + background).saturated().gamma_corrected(2.2), y flipped.
@@ -23,11 +25,13 @@ static constexpr float kAdaptiveThreshold = 0.025f;
 static constexpr int kAdaptiveMaxRounds = 32;
 
 // setup.rs:46-169; `fractal` 0 = Mandelbox (the reference scene), 1 = authored Mandelbulb
-static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens) {
+// trap: the fractal's albedo generator (--orbit-trap), NULL = the reference's constant grey
+static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens, const OrbitTrapAlbedo* trap = nullptr) {
   if (volume) world.volume_params = VolumeParams{true, true, 0.25f, 0.035f};                      // :55-60
   const MaterialHandle sky = world.materials.add_material(Sky(Srgb(0.3f, 0.4f, 0.6f), Srgb(0.2f, 0.3f, 0.6f) * 0.05f));  // :63-69
   world.hitables.push(Sphere(Vec3(0, 0, 0), WORLD_RADIUS, sky));                                  // :71
-  const MaterialHandle grey = world.materials.add_material(Dielectric::new_remap(Srgb(0.2f, 0.2f, 0.2f), 0.6f));        // :76
+  const MaterialHandle grey = trap ? world.materials.add_material(Dielectric::new_remap(*trap, 0.6f))
+                                   : world.materials.add_material(Dielectric::new_remap(Srgb(0.2f, 0.2f, 0.2f), 0.6f));  // :76
   if (fractal == 0)
     world.hitables.push(TracedSDF(MandelBox(FRACTAL_ITERATIONS, BoxFold(1.0f), SphereFold(0.01f, 1.9f), -2.1f), grey));  // :78-86
   else
@@ -68,6 +72,8 @@ int main(int argc, char** argv) {
   int max_rounds = kAdaptiveMaxRounds;
   bool res_set = false, samples_set = false, bounces_set = false;
   const char *out = nullptr, *dump = nullptr, *dump_scene = nullptr;
+  bool orbit_trap = false;
+  OrbitTrapAlbedo trap{0.0f, 1.0f, Srgb(0, 0, 0), Srgb(0, 0, 0)};
   for (int i = 1; i < argc; ++i) {
     if (!strcmp(argv[i], "--config") && i + 1 < argc) config = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--res") && i + 2 < argc) W = atoi(argv[++i]), H = atoi(argv[++i]), res_set = true;
@@ -79,9 +85,14 @@ int main(int argc, char** argv) {
     else if (!strcmp(argv[i], "--denoise") && i + 1 < argc) denoise = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--adaptive") && i + 1 < argc) adaptive = true, threshold = (float)atof(argv[++i]);
     else if (!strcmp(argv[i], "--rounds") && i + 1 < argc) max_rounds = atoi(argv[++i]);
-    else {
+    else if (!strcmp(argv[i], "--orbit-trap") && i + 8 < argc) {
+      float v[8];
+      for (int k = 0; k < 8; ++k) v[k] = (float)atof(argv[++i]);
+      trap = OrbitTrapAlbedo{v[0], v[1], Srgb(v[2], v[3], v[4]), Srgb(v[5], v[6], v[7])};
+      orbit_trap = true;
+    } else {
       fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] "
-                      "[--denoise L] [--out f.ppm] [--dump f.bin]\n");
+                      "[--denoise L] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out f.ppm] [--dump f.bin]\n");
       return 2;
     }
   }
@@ -90,13 +101,15 @@ int main(int argc, char** argv) {
   static const int cfg_res[6][2] = {{0, 0}, {256, 256}, {1024, 1024}, {1920, 1080}, {2048, 2048}, {7680, 4320}};
   static const int cfg_samples[6] = {0, 1, 32, 128, 64, 256}, cfg_bounces[6] = {0, 2, 4, 8, 4, 8};
   if (config < 1 || config > 5) { fprintf(stderr, "config must be 1..5\n"); return 2; }
+  if (orbit_trap && config == 1) { fprintf(stderr, "--orbit-trap colours the fractal of configs 2-5\n"); return 2; }
   if (!res_set) W = cfg_res[config][0], H = cfg_res[config][1];
   if (!samples_set) samples = cfg_samples[config];
   if (!bounces_set) bounces = cfg_bounces[config];
   try {
     World world;
     const CameraHandle camera = config == 1 ? setup_single_sphere(world, (float)W, (float)H)
-                                            : setup(world, (float)W, (float)H, config == 4, config == 3 ? 0 : 1, config == 4);
+                                            : setup(world, (float)W, (float)H, config == 4, config == 3 ? 0 : 1, config == 4,
+                                                    orbit_trap ? &trap : nullptr);
     if (dump_scene) {  // flattened World as raw PODs (no GPU needed): hitables | materials | lights | camera | volume
       FILE* f = fopen(dump_scene, "wb");
       if (!f) { perror(dump_scene); return 1; }

@@ -40,22 +40,41 @@ using MaterialHandle = int;
 using CameraHandle = int;
 
 // ---- materials (material.rs) ------------------------------------------------------------
+// An albedo generator (rayn's albedo_gen, material.rs:75-83) that colours an SDF surface by orbit trap: the trap value at the
+// hit, mapped from [trap_lo, trap_hi] onto lo .. hi and clamped; analytic spheres get hi (include/rayn_b200.h, RaynAlbedoTrap).
+struct OrbitTrapAlbedo {
+  float trap_lo, trap_hi;
+  Srgb lo, hi;
+};
 struct Material {
   RaynMaterial pod{};
+  bool has_trap = false;
+  RaynAlbedoTrap trap{};  // material index filled in by MaterialStore::add_material
+ protected:
+  void set_albedo(const Srgb& a) { a.store(pod.albedo); }
+  void set_albedo(const OrbitTrapAlbedo& t) {  // the constant is albedo_hi, what a trap material gives on analytic spheres
+    t.hi.store(pod.albedo);
+    has_trap = true;
+    trap.trap_lo = t.trap_lo, trap.trap_hi = t.trap_hi;
+    t.lo.store(trap.albedo_lo), t.hi.store(trap.albedo_hi);
+  }
 };
 struct Lambertian : Material {  // material.rs:91-100
-  explicit Lambertian(Srgb albedo) {
+  template <class A>
+  explicit Lambertian(A albedo) {
     pod.kind = RAYN_MATERIAL_LAMBERTIAN;
-    albedo.store(pod.albedo);
+    set_albedo(albedo);
   }
 };
 struct Dielectric : Material {  // material.rs:150-175
-  Dielectric(Srgb albedo, float roughness_exponent) {
+  template <class A>
+  Dielectric(A albedo, float roughness_exponent) {
     pod.kind = RAYN_MATERIAL_DIELECTRIC;
-    albedo.store(pod.albedo);
+    set_albedo(albedo);
     pod.roughness = roughness_exponent;
   }
-  static Dielectric new_remap(Srgb albedo, float roughness) {  // :167-174
+  template <class A>
+  static Dielectric new_remap(A albedo, float roughness) {  // :167-174
     float r = 1.0f - roughness;
     r = 1.0f + r * r * r * r * 300.0f;
     return Dielectric(albedo, r);
@@ -78,9 +97,15 @@ struct Emissive : Material {  // material.rs:451-469
 };
 struct MaterialStore {  // material.rs:58-73
   std::vector<RaynMaterial> items;
+  std::vector<RaynAlbedoTrap> traps;  // orbit-trap albedos, one per material that has one (rayn_b200_set_albedo_traps)
   MaterialHandle add_material(const Material& m) {
     items.push_back(m.pod);
-    return (MaterialHandle)items.size() - 1;
+    const MaterialHandle h = (MaterialHandle)items.size() - 1;
+    if (m.has_trap) {
+      traps.push_back(m.trap);
+      traps.back().material = h;
+    }
+    return h;
   }
 };
 
@@ -328,6 +353,8 @@ class Film {
                            world.volume_params.coeff_extinction};
     sc.consts = world.consts;
     check(rayn_b200_upload_scene(ctx_, &sc), ctx_);
+    if (!world.materials.traps.empty())
+      check(rayn_b200_set_albedo_traps(ctx_, (int32_t)world.materials.traps.size(), world.materials.traps.data()), ctx_);
   }
   RaynFrameDesc frame_desc(const PathTracingIntegrator& integrator, int tile_w, int tile_h, int frame, float t0, float t1, int samples, int sets_1d,
                            int sets_2d) const {

@@ -86,9 +86,40 @@ def _seq(x):
 
 
 # ---- materials (material.rs) ---------------------------------------------------------------
+class OrbitTrapAlbedo:
+    """An albedo generator (rayn's `albedo_gen: WShadingParamGenerator<WSrgb>`, material.rs:75-83) that colours an SDF surface
+    by orbit trap: the smallest squared radius the distance estimator's iteration reaches at the hit point (Mandelbox: the r2
+    its sphere fold divides by; Mandelbulb: |w|^2), mapped linearly from [trap_lo, trap_hi] onto albedo_lo .. albedo_hi and
+    clamped.  Hits on analytic spheres take albedo_hi.  The exact statement is in include/rayn_b200.h (RaynAlbedoTrap).
+    Pass it as the albedo of Lambertian(...), Dielectric(...) or Dielectric.new_remap(...)."""
+
+    def __init__(self, trap_lo, trap_hi, albedo_lo, albedo_hi):
+        self.trap_lo, self.trap_hi = f32(trap_lo), f32(trap_hi)
+        self.albedo_lo, self.albedo_hi = _arr(albedo_lo), _arr(albedo_hi)
+        if not (np.isfinite(self.trap_lo) and np.isfinite(self.trap_hi) and self.trap_lo < self.trap_hi):
+            raise ValueError(f"OrbitTrapAlbedo needs finite trap_lo < trap_hi, got {trap_lo}, {trap_hi}")
+        if not (np.isfinite(self.albedo_lo).all() and np.isfinite(self.albedo_hi).all()):
+            raise ValueError("OrbitTrapAlbedo needs finite albedos")
+
+    def trap_desc(self, material):
+        t = L.RaynAlbedoTrap()
+        t.material = int(material)
+        t.trap_lo, t.trap_hi = float(self.trap_lo), float(self.trap_hi)
+        t.albedo_lo[:] = self.albedo_lo.tolist()
+        t.albedo_hi[:] = self.albedo_hi.tolist()
+        return t
+
+
+def _albedo(albedo):
+    """-> (constant albedo[3], OrbitTrapAlbedo or None).  A trap material's constant is albedo_hi (what analytic spheres get)."""
+    if isinstance(albedo, OrbitTrapAlbedo):
+        return albedo.albedo_hi.copy(), albedo
+    return _arr(albedo), None
+
+
 class Lambertian:  # material.rs:91-100
     def __init__(self, albedo):
-        self.albedo = _arr(albedo)
+        self.albedo, self.albedo_gen = _albedo(albedo)
 
     def flatten(self):
         m = L.RaynMaterial()
@@ -99,7 +130,7 @@ class Lambertian:  # material.rs:91-100
 
 class Dielectric:  # material.rs:150-175
     def __init__(self, albedo, roughness_exponent):
-        self.albedo = _arr(albedo)
+        self.albedo, self.albedo_gen = _albedo(albedo)
         self.roughness = f32(roughness_exponent)
 
     @staticmethod
@@ -364,6 +395,10 @@ class World:  # world.rs:7-13
         d.consts.max_marches = int(self.consts.max_marches)
         d.consts.max_vis_marches = int(self.consts.max_vis_marches)
         return d, (hit, mat, lig)
+
+    def albedo_traps(self):
+        """-> [RaynAlbedoTrap]: one entry per material whose albedo is an OrbitTrapAlbedo (rayn_b200_set_albedo_traps)."""
+        return [m.albedo_gen.trap_desc(i) for i, m in enumerate(self.materials.items) if getattr(m, "albedo_gen", None) is not None]
 
 
 class PathTracingIntegrator:  # integrator.rs:33-45
