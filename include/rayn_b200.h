@@ -317,6 +317,28 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* frame,
 
 int32_t rayn_b200_get_stats(const RaynContext* ctx, RaynStats* out);
 
+/* ---- first-hit albedo plane: an AOV for denoisers (rayn_b200_film_denoise_albedo, or an external one beside the
+ * normal plane) -----------------------------------------------------------------------------------------------------
+ * albedo[3*W*H] (row-major, y up, like the film planes) in memory space `space` (RaynMemSpace).  In float, no contraction:
+ * for every pixel of the tile grid (film.rs:399-404) and every camera sample s = 0..spp-1 (spp = 4*frame->samples), the
+ * ray render_frame generates for that sample (same tables, scramble, filter, time and lens; the camera takes the time of
+ * lane 0 of its 4-sample packet) is traced to its closest hit with the DEPTH-0 fold of render_frame (hitable.rs:170-198,
+ * threshold film.rs:540-551), which is render_frame's depth-0 hit exactly (moving spheres at lane 0's time of the extend
+ * packet, which at depth 0 is samples 4k..4k+3 of the pixel).  Its albedo a_s is
+ *   Lambertian or Dielectric hit: the albedo the BSDF reads at depth 0, i.e. RaynMaterial.albedo, or for a material with
+ *     an orbit trap lo*(1 - s') + hi*s' (RaynAlbedoTrap) with s' = trap_coord(trap(p)), p = dir.mul_add(t, origin) the hit
+ *     point (ray.rs:22-24), s' = 1 on an analytic sphere;
+ *   Sky or Emissive hit, or nothing hit: (0, 0, 0).
+ * albedo[3p+c] = (((+0 + a_0[c]) + a_1[c]) + ... + a_{spp-1}[c]) / (float)spp, summed in ascending sample order; pixels
+ * outside the tile grid are 0.  frame->tile_list / tile_offset / tile_stride are ignored (the whole grid is rendered); all
+ * other frame checks are render_frame's.  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; replaces RaynStats
+ * like a render (k_albedo_paths counts under RAYN_K_NORMALS, k_albedo_resolve under RAYN_K_RESOLVE); never captured into a
+ * CUDA graph, and later renders are unaffected.
+ * Property (tested): if every Lambertian / Dielectric material has albedo (1, 1, 1) and there are no traps, every channel
+ * equals render_frame's alpha plane bit for bit, for the same frame: alpha is nA / spp with nA the count of depth-0
+ * Lambertian / Dielectric hits, and a sum of nA ones is nA exactly.                                                 */
+int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, float* albedo /* [3*W*H] */, int32_t space);
+
 /* ---- multi-GPU: film tiles shard across GPUs, NCCL only for the final film gather -------------------------
  * The reference's only parallelism is one rayon task per tile over shared read-only state (film.rs:640-649); the
  * multi-GPU form of that is one context per GPU, each rendering the tiles `(tile_x + tile_y) % world == rank`
@@ -405,6 +427,15 @@ typedef struct RaynDenoiseDesc {
 } RaynDenoiseDesc;
 int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* desc, int32_t width, int32_t height,
                                const RaynFilmPlanes* in, const RaynFilmPlanes* out);
+/* The same filter with an albedo guide (e.g. rayn_b200_render_albedo's plane): per tap, with
+ *   dl2 = (dr*dr + dg*dg) + db*db of albedo_q - albedo_p,   il = 1/sigma_albedo^2 (the same at every level),
+ *   e = ((dc2*ic_i + dn2*in) + da2*ia) + dl2*il
+ * and everything else as in rayn_b200_film_denoise (sigma, skip, aliasing, space and asynchrony rules).  `albedo` is a
+ * [3*W*H] plane in in->space; NULL is RAYN_ERR_INVALID_ARG.  sigma_albedo must be > 0 with a finite 1/sigma^2; at +inf the
+ * term is NOT added, and the call equals rayn_b200_film_denoise bit for bit.  A tap whose albedo has a non-finite
+ * component gets a NaN e (skipped) or e = +inf (weight +0).                                                         */
+int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_albedo, const float* albedo,
+                                      int32_t width, int32_t height, const RaynFilmPlanes* in, const RaynFilmPlanes* out);
 
 /* ---- progressive / adaptive rendering: a device film accumulator refined in sample rounds -----------------------
  * Per-tile stopping rule after Dammertz, Hanika, Keller, Lensch (WSCG 2009; PAPERS.md): a tile's error compares the

@@ -153,6 +153,9 @@ SYMBOLS = {
     "rayn_b200_film_unpack_tiles": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(i32), i32, C.c_void_p, C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_film_postprocess": (i32, [C.c_void_p, i32, i32, i32, C.POINTER(RaynFilmPlanes), C.c_void_p, i32]),
     "rayn_b200_film_denoise": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_film_denoise_albedo": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, C.c_void_p, i32, i32, C.POINTER(RaynFilmPlanes),
+                                            C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_render_albedo": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), C.c_void_p, i32]),
     "rayn_b200_accum_create": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(C.c_void_p)]),
     "rayn_b200_accum_destroy": (None, [C.c_void_p]),
     "rayn_b200_accum_round": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynAdaptiveDesc), C.POINTER(i32)]),

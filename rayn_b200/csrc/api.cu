@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "rt_accum.cuh"
+#include "rt_albedo.cuh"
 #include "rt_denoise.cuh"
 #include "rt_kernels.cuh"
 #ifdef RAYN_LEGACY_KERNELS
@@ -551,15 +552,19 @@ int64_t rayn_b200_debug_read_queue_log(RaynContext* ctx, int32_t* out, int64_t c
 
 }  // extern "C"
 
-// Enqueues one render on the context's stream.  Nothing here waits for the GPU (except the debug queue log), so a single
-// host thread can keep several GPUs busy (render_frame_multi).  tiles_override replaces the frame's own tile selection.
-// dev_planes_out (optional) receives the device-space planes the film was rendered into.
-static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
-                              RaynFilmPlanes* dev_planes_out) {
-  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
-  if (ctx->pending) return fail(ctx, RAYN_ERR_INVALID_ARG, "a render is already in flight on this context");
-  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "render_frame before upload_scene");
-  if (!f || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/out is NULL");
+// ---- the stages a render and the albedo pass (rayn_b200_render_albedo) share ----------------------------------------
+// What a render derives from its frame (frame_check) and from the uploaded scene (scene_plan) before it launches anything.
+struct FramePlan {
+  DevFrame fr;
+  int R, QS, np, wpc;  // paths and shading slots per tile; k_resolve's padded spp and warps per CTA
+  int n_sdf, sdf_idx[RAYN_MAX_HITABLES];
+  bool simple, motion, traps, fold_all, volume_on;
+  int fold_pre, n_fold, ns, seg_per_path, lc_ns;
+};
+
+// The frame checks of render_frame and the DevFrame of the frame (tables not uploaded yet).  tiles_given: the caller picks
+// the tiles itself, so tile_offset / tile_stride are not checked.
+static int32_t frame_check(RaynContext* ctx, const RaynFrameDesc* f, bool tiles_given, FramePlan* P) {
   if (f->width <= 0 || f->height <= 0 || f->tile_w <= 0 || f->tile_h <= 0 || f->samples <= 0 || f->max_bounces < 0)
     return fail(ctx, RAYN_ERR_INVALID_ARG, "bad frame geometry");
   if (f->volume_marches != 2)
@@ -570,18 +575,19 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     return fail(ctx, RAYN_ERR_INVALID_ARG, "sample tables too small: have %d/%d sets, path needs %d/%d", f->sets_1d, f->sets_2d, need1, need2);
   if (!f->samples_1d || !f->samples_2d || !f->scramble || !f->fis_inverse_cdf) return fail(ctx, RAYN_ERR_INVALID_ARG, "NULL input table");
   const int stride = f->tile_stride > 0 ? f->tile_stride : 1;
-  if (!tiles_override && !f->tile_list && (f->tile_offset < 0 || f->tile_offset >= stride))
+  if (!tiles_given && !f->tile_list && (f->tile_offset < 0 || f->tile_offset >= stride))
     return fail(ctx, RAYN_ERR_INVALID_ARG, "tile_offset %d not in [0,%d)", f->tile_offset, stride);
   if (mb >= TERM_MAX_DEPTH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "max_bounces > %d", TERM_MAX_DEPTH - 1);
   const int64_t R64 = (int64_t)f->tile_w * f->tile_h * spp;
   const int n_hit = ctx->scene.n_hit;
   if (R64 + 4 * n_hit >= TERM_MAX_SLOTS)
     return fail(ctx, RAYN_ERR_UNSUPPORTED, "tile_w*tile_h*spp = %lld exceeds the 2^%d slot key space", (long long)R64, TERM_DEPTH_SHIFT);
-  int np = 32;
+  int& np = P->np;
+  np = 32;
   while (np < spp) np <<= 1;
-  const int wpc = resolve_warps_per_cta(np);
+  const int wpc = P->wpc = resolve_warps_per_cta(np);
   if (wpc < 1 || np > 65536) return fail(ctx, RAYN_ERR_UNSUPPORTED, "spp = %d: the film resolve holds 6 B per sample of a pixel in shared memory (max 32768 spp)", spp);
-  const int R = (int)R64, QS = R + 4 * n_hit;
+  P->R = (int)R64, P->QS = P->R + 4 * n_hit;
   CU(cudaSetDevice(ctx->device));
   {  // a previous call that failed half way through a graph capture must not leave the stream capturing
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -593,13 +599,149 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     cudaGetLastError();
   }
 
-  DevFrame fr;
+  DevFrame& fr = P->fr;
   fr.W = f->width, fr.H = f->height, fr.tile_w = f->tile_w, fr.tile_h = f->tile_h;
   fr.samples = f->samples, fr.spp = spp, fr.max_bounces = mb, fr.vm = vm;
   tile_grid_of(f->width, f->height, f->tile_w, f->tile_h, &fr.ntx, &fr.nty);
   fr.sets_1d = f->sets_1d, fr.sets_2d = f->sets_2d;
   fr.t0 = f->t0, fr.t1 = f->t1;
+  return RAYN_OK;
+}
 
+// The sample tables, scramble and filter table on the device: host-space inputs are copied into the context's staging.
+static int32_t upload_tables(RaynContext* ctx, const RaynFrameDesc* f, DevFrame* frp) {
+  DevFrame& fr = *frp;
+  const int spp = fr.spp;
+  cudaStream_t st = ctx->stream;
+  const size_t n1 = (size_t)spp * f->sets_1d, n2 = (size_t)2 * spp * f->sets_2d, npx = (size_t)f->width * f->height;
+  if (f->input_space == RAYN_MEM_HOST) {
+    CU(regrow(&ctx->d_s1, &ctx->cap_s1, n1));
+    CU(regrow(&ctx->d_s2, &ctx->cap_s2, n2));
+    CU(regrow(&ctx->d_scr, &ctx->cap_scr, npx));
+    CU(cudaMemcpyAsync(ctx->d_s1, f->samples_1d, n1 * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_s2, f->samples_2d, n2 * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_scr, f->scramble, npx * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_fis, f->fis_inverse_cdf, RAYN_FIS_TABLE_SIZE * 4, cudaMemcpyHostToDevice, st));
+    fr.s1 = ctx->d_s1, fr.s2 = ctx->d_s2, fr.scramble = ctx->d_scr, fr.fis = ctx->d_fis;
+  } else {
+    fr.s1 = f->samples_1d, fr.s2 = f->samples_2d, fr.scramble = f->scramble, fr.fis = f->fis_inverse_cdf;
+  }
+  return RAYN_OK;
+}
+
+// Which kernels the scene needs and how the closest-hit fold is split between them.
+static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
+  const int n_hit = ctx->scene.n_hit, vm = P->fr.vm;
+  int& n_sdf = P->n_sdf;
+  int* sdf_idx = P->sdf_idx;
+  n_sdf = 0;
+  for (int i = 0; i < n_hit; ++i)
+    if (ctx->scene.hit[i].kind != RAYN_HITABLE_SPHERE) sdf_idx[n_sdf++] = i;
+  const bool simple = P->simple = (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) != 0;
+  bool& motion = P->motion;
+  motion = false;  // time-varying sphere centres need the packet's lane-0 time: only the product kernels plumb it
+  for (int i = 0; i < n_hit; ++i)
+    motion |= ctx->scene.hit[i].kind == RAYN_HITABLE_SPHERE && (ctx->scene.hit[i].center_velocity[0] != 0.0f || ctx->scene.hit[i].center_velocity[1] != 0.0f ||
+                                                                 ctx->scene.hit[i].center_velocity[2] != 0.0f);
+  if (motion && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "time-varying sphere centres are not supported by the legacy test kernels");
+  const bool traps = P->traps = ctx->scene.trap_mask != 0u;
+  if (traps && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "orbit-trap albedos are not supported by the legacy test kernels");
+  // leading analytic spheres run inside raygen / shade_post (rt_kernels.cuh::fold_head); -1 = not folded (moving spheres need
+  // the extend packet's lane-0 time; the legacy test kernels do the whole fold themselves)
+  int& fold_pre = P->fold_pre;
+  fold_pre = -1;
+  if (!motion && !simple) {
+    fold_pre = 0;
+    while (fold_pre < n_hit && ctx->scene.hit[fold_pre].kind == RAYN_HITABLE_SPHERE) ++fold_pre;
+  }
+  // Scenes of the shape [spheres] Mandelbox [spheres] (setup.rs) fold ALL analytic spheres into the producing kernel and march
+  // the SDF last, against the nearest sphere: one gather of every live ray per depth less (no k_extend_spheres
+  // launch) and shorter marches for rays that end on an emitter.  The result is the reference's fold bit for bit
+  // (proof in rt_kernels.cuh at k_extend_march: it needs a distance estimator that is never negative, i.e. the Mandelbox -
+  // sqrt(m) / |dr| - so that a march's t never decreases, and the first-index-wins tie rule, which the kernel applies).
+  const bool fold_all = P->fold_all = fold_pre >= 0 && n_sdf == 1 && ctx->scene.hit[sdf_idx[0]].kind == RAYN_HITABLE_MANDELBOX && !(ctx->flags & RAYN_FLAG_NO_FOLD_ALL);
+  P->n_fold = fold_all ? ctx->scene.n_sph : fold_pre;  // leading spheres are the first fold_pre entries of the compact sphere list
+  const bool volume_on = P->volume_on = ctx->scene.vol.has_scattering != 0 && ctx->scene.n_lights > 0;
+  const int ns = P->ns = volume_on ? 4 * (1 + vm) : 4;               // light samples per path per depth
+  P->seg_per_path = simple ? 0 : ns * n_sdf;          // worst case shadow segments per path per depth, all SDF queues
+  P->lc_ns = simple ? 0 : ns;                         // stored light contributions per path per depth
+  return RAYN_OK;
+}
+
+// Pass size for n_tiles tiles (as many tiles per pass as the path budget and free device memory allow), and the pass buffers.
+static int32_t size_pass(RaynContext* ctx, const FramePlan& P, size_t n_tiles, int* out_tiles_per_pass) {
+  const int R = P.R, QS = P.QS, n_sdf = P.n_sdf, ns = P.ns, seg_per_path = P.seg_per_path, lc_ns = P.lc_ns;
+  const bool traps = P.traps;
+  const size_t bpp = pass_bytes_per_path(R, QS, seg_per_path, lc_ns, traps);
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  const size_t budget = (size_t)((double)(free_b + ctx->pass_bytes) * 0.90);
+  int64_t max_paths = std::min<int64_t>(ctx->cap_paths, (int64_t)(budget / bpp));
+  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, ((int64_t)1 << 27) - 1);          // owner path index is packed with the sample bit (<< 4)
+  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, (int64_t)INT_MAX / std::max(ns, 1));  // 32-bit queue cursors per SDF
+  int& tiles_per_pass = *out_tiles_per_pass;
+  tiles_per_pass = (int)std::max<int64_t>(1, max_paths / R);
+  tiles_per_pass = std::min(tiles_per_pass, 65535);
+  tiles_per_pass = std::min<int>(tiles_per_pass, (int)std::max<size_t>(n_tiles, 1));
+  int32_t rc;
+  while ((rc = ensure_pass(ctx, tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps)) == RAYN_ERR_OOM && tiles_per_pass > 1)
+    tiles_per_pass = (tiles_per_pass + 1) / 2;  // fragmentation / another tenant: retry with half the pass
+  return rc;
+}
+
+// One depth's closest-hit stage (the non-legacy kernels): k_scan_live, then the fold over the live rays of the pass.
+// sph_grid: the resident grid of k_extend_spheres.
+static int32_t extend_enqueue(RaynContext* ctx, const FramePlan& P, const PassBufs& pb, const Thr& thr, unsigned sph_grid) {
+  cudaStream_t st = ctx->stream;
+  const int n_hit = ctx->scene.n_hit, fold_pre = P.fold_pre;
+  const bool fold_all = P.fold_all, motion = P.motion;
+  timed_begin(ctx, RAYN_K_MISC);
+  k_scan_live<<<1, SCAN_T, 0, st>>>(pb, ctx->d_batch_prefix, ctx->d_work_ctr);
+  timed_end(ctx, RAYN_K_MISC);
+  // fold order of hitable.rs:177-198: runs of spheres as coherent kernels, each SDF as a persistent march.  The
+  // spheres before the first SDF were already folded in by the kernel that produced the rays (fold_pre >= 0).
+  int k = fold_pre >= 0 ? fold_pre : 0, first_kernel = fold_pre >= 0 ? 0 : 1, n_march = 0;
+  while (k < n_hit || first_kernel) {
+    int e = k;
+    while (e < n_hit && ctx->scene.hit[e].kind == RAYN_HITABLE_SPHERE) ++e;
+    if ((e > k || first_kernel) && !fold_all) {
+      timed_begin(ctx, RAYN_K_EXTEND_SPHERES);
+      k_extend_spheres<<<sph_grid, EXT_BATCH, 0, st>>>(ctx->scene, pb, k, e, first_kernel, motion ? 1 : 0, ctx->d_batch_prefix, ctx->d_work_ctr + WC_SPHERES + k);
+      timed_end(ctx, RAYN_K_EXTEND_SPHERES);
+      first_kernel = 0;
+    }
+    if (e < n_hit) {
+      if (n_march++ > 0) CU(cudaMemsetAsync(ctx->d_work_ctr + WC_EXTEND, 0, sizeof(int), st));
+      const int v = ctx->sdf_var[e];
+      timed_begin(ctx, RAYN_K_EXTEND);
+      const int sf = fold_all ? 1 : 0;
+      if (thr.is_const)
+        DISPATCH_SDFV(v, (k_extend_march<V, true><<<ctx->n_sm * ctx->occ_ext[1][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
+      else
+        DISPATCH_SDFV(v, (k_extend_march<V, false><<<ctx->n_sm * ctx->occ_ext[0][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
+      timed_end(ctx, RAYN_K_EXTEND);
+      ++e;
+    }
+    k = e;
+  }
+  return RAYN_OK;
+}
+
+// Enqueues one render on the context's stream.  Nothing here waits for the GPU (except the debug queue log), so a single
+// host thread can keep several GPUs busy (render_frame_multi).  tiles_override replaces the frame's own tile selection.
+// dev_planes_out (optional) receives the device-space planes the film was rendered into.
+static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
+                              RaynFilmPlanes* dev_planes_out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (ctx->pending) return fail(ctx, RAYN_ERR_INVALID_ARG, "a render is already in flight on this context");
+  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "render_frame before upload_scene");
+  if (!f || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/out is NULL");
+  FramePlan P;
+  int32_t rc = frame_check(ctx, f, tiles_override != nullptr, &P);
+  if (rc) return rc;
+  DevFrame& fr = P.fr;
+  const int spp = fr.spp, mb = fr.max_bounces, np = P.np, wpc = P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit;
+  const int stride = f->tile_stride > 0 ? f->tile_stride : 1;
   std::vector<int>& my_tiles = ctx->job_tiles;
   my_tiles.clear();
   if (tiles_override) {
@@ -625,19 +767,8 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   if (f->input_space == RAYN_MEM_DEVICE || out->space == RAYN_MEM_DEVICE) CU(cudaDeviceSynchronize());
   CU(cudaEventRecord(ctx->ev0, st));
 
-  const size_t n1 = (size_t)spp * f->sets_1d, n2 = (size_t)2 * spp * f->sets_2d, npx = (size_t)f->width * f->height;
-  if (f->input_space == RAYN_MEM_HOST) {
-    CU(regrow(&ctx->d_s1, &ctx->cap_s1, n1));
-    CU(regrow(&ctx->d_s2, &ctx->cap_s2, n2));
-    CU(regrow(&ctx->d_scr, &ctx->cap_scr, npx));
-    CU(cudaMemcpyAsync(ctx->d_s1, f->samples_1d, n1 * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_s2, f->samples_2d, n2 * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_scr, f->scramble, npx * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_fis, f->fis_inverse_cdf, RAYN_FIS_TABLE_SIZE * 4, cudaMemcpyHostToDevice, st));
-    fr.s1 = ctx->d_s1, fr.s2 = ctx->d_s2, fr.scramble = ctx->d_scr, fr.fis = ctx->d_fis;
-  } else {
-    fr.s1 = f->samples_1d, fr.s2 = f->samples_2d, fr.scramble = f->scramble, fr.fis = f->fis_inverse_cdf;
-  }
+  if ((rc = upload_tables(ctx, f, &fr))) return rc;
+  const size_t npx = (size_t)f->width * f->height;
   float *p_color, *p_alpha, *p_bg, *p_normal;
   if (out->space == RAYN_MEM_HOST) {
     CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 10));
@@ -654,52 +785,13 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     dev_planes_out->space = RAYN_MEM_DEVICE;
   }
 
-  int n_sdf = 0;
-  int sdf_idx[RAYN_MAX_HITABLES];
-  for (int i = 0; i < n_hit; ++i)
-    if (ctx->scene.hit[i].kind != RAYN_HITABLE_SPHERE) sdf_idx[n_sdf++] = i;
-  const bool simple = (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) != 0;
-  bool motion = false;  // time-varying sphere centres need the packet's lane-0 time: only the product kernels plumb it
-  for (int i = 0; i < n_hit; ++i)
-    motion |= ctx->scene.hit[i].kind == RAYN_HITABLE_SPHERE && (ctx->scene.hit[i].center_velocity[0] != 0.0f || ctx->scene.hit[i].center_velocity[1] != 0.0f ||
-                                                                 ctx->scene.hit[i].center_velocity[2] != 0.0f);
-  if (motion && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "time-varying sphere centres are not supported by the legacy test kernels");
-  const bool traps = ctx->scene.trap_mask != 0u;
-  if (traps && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "orbit-trap albedos are not supported by the legacy test kernels");
-  // leading analytic spheres run inside raygen / shade_post (rt_kernels.cuh::fold_head); -1 = not folded (moving spheres need
-  // the extend packet's lane-0 time; the legacy test kernels do the whole fold themselves)
-  int fold_pre = -1;
-  if (!motion && !simple) {
-    fold_pre = 0;
-    while (fold_pre < n_hit && ctx->scene.hit[fold_pre].kind == RAYN_HITABLE_SPHERE) ++fold_pre;
-  }
-  // Scenes of the shape [spheres] Mandelbox [spheres] (setup.rs) fold ALL analytic spheres into the producing kernel and march
-  // the SDF last, against the nearest sphere: one gather of every live ray per depth less (no k_extend_spheres
-  // launch) and shorter marches for rays that end on an emitter.  The result is the reference's fold bit for bit
-  // (proof in rt_kernels.cuh at k_extend_march: it needs a distance estimator that is never negative, i.e. the Mandelbox -
-  // sqrt(m) / |dr| - so that a march's t never decreases, and the first-index-wins tie rule, which the kernel applies).
-  const bool fold_all = fold_pre >= 0 && n_sdf == 1 && ctx->scene.hit[sdf_idx[0]].kind == RAYN_HITABLE_MANDELBOX && !(ctx->flags & RAYN_FLAG_NO_FOLD_ALL);
-  const int n_fold = fold_all ? ctx->scene.n_sph : fold_pre;  // leading spheres are the first fold_pre entries of the compact sphere list
-  const bool volume_on = ctx->scene.vol.has_scattering != 0 && ctx->scene.n_lights > 0;
-  const int ns = volume_on ? 4 * (1 + vm) : 4;               // light samples per path per depth
-  const int seg_per_path = simple ? 0 : ns * n_sdf;          // worst case shadow segments per path per depth, all SDF queues
-  const int lc_ns = simple ? 0 : ns;                         // stored light contributions per path per depth
+  if ((rc = scene_plan(ctx, &P))) return rc;
+  const int n_sdf = P.n_sdf, n_fold = P.n_fold, lc_ns = P.lc_ns;
+  const int* sdf_idx = P.sdf_idx;
+  const bool simple = P.simple, motion = P.motion, traps = P.traps, volume_on = P.volume_on;
 
-  // pass size: as many tiles as the requested path budget AND free device memory allow
-  const size_t bpp = pass_bytes_per_path(R, QS, seg_per_path, lc_ns, traps);
-  size_t free_b = 0, total_b = 0;
-  CU(cudaMemGetInfo(&free_b, &total_b));
-  const size_t budget = (size_t)((double)(free_b + ctx->pass_bytes) * 0.90);
-  int64_t max_paths = std::min<int64_t>(ctx->cap_paths, (int64_t)(budget / bpp));
-  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, ((int64_t)1 << 27) - 1);          // owner path index is packed with the sample bit (<< 4)
-  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, (int64_t)INT_MAX / std::max(ns, 1));  // 32-bit queue cursors per SDF
-  int tiles_per_pass = (int)std::max<int64_t>(1, max_paths / R);
-  tiles_per_pass = std::min(tiles_per_pass, 65535);
-  tiles_per_pass = std::min<int>(tiles_per_pass, (int)std::max<size_t>(my_tiles.size(), 1));
-  int32_t rc;
-  while ((rc = ensure_pass(ctx, tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps)) == RAYN_ERR_OOM && tiles_per_pass > 1)
-    tiles_per_pass = (tiles_per_pass + 1) / 2;  // fragmentation / another tenant: retry with half the pass
-  if (rc) return rc;
+  int tiles_per_pass;
+  if ((rc = size_pass(ctx, P, my_tiles.size(), &tiles_per_pass))) return rc;
   PassBufs pb = ctx->pb;
   pb.R = R, pb.QS = QS, pb.tile_ids = ctx->d_tile_ids;
   pb.lc_ns = lc_ns;
@@ -764,35 +856,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
         timed_end(ctx, RAYN_K_EXTEND);
 #endif
       } else {
-        timed_begin(ctx, RAYN_K_MISC);
-        k_scan_live<<<1, SCAN_T, 0, st>>>(pb, ctx->d_batch_prefix, ctx->d_work_ctr);
-        timed_end(ctx, RAYN_K_MISC);
-        // fold order of hitable.rs:177-198: runs of spheres as coherent kernels, each SDF as a persistent march.  The
-        // spheres before the first SDF were already folded in by the kernel that produced the rays (fold_pre >= 0).
-        int k = fold_pre >= 0 ? fold_pre : 0, first_kernel = fold_pre >= 0 ? 0 : 1, n_march = 0;
-        while (k < n_hit || first_kernel) {
-          int e = k;
-          while (e < n_hit && ctx->scene.hit[e].kind == RAYN_HITABLE_SPHERE) ++e;
-          if ((e > k || first_kernel) && !fold_all) {
-            timed_begin(ctx, RAYN_K_EXTEND_SPHERES);
-            k_extend_spheres<<<resident(ctx->occ_sph), EXT_BATCH, 0, st>>>(ctx->scene, pb, k, e, first_kernel, motion ? 1 : 0, ctx->d_batch_prefix, ctx->d_work_ctr + WC_SPHERES + k);
-            timed_end(ctx, RAYN_K_EXTEND_SPHERES);
-            first_kernel = 0;
-          }
-          if (e < n_hit) {
-            if (n_march++ > 0) CU(cudaMemsetAsync(ctx->d_work_ctr + WC_EXTEND, 0, sizeof(int), st));
-            const int v = ctx->sdf_var[e];
-            timed_begin(ctx, RAYN_K_EXTEND);
-            const int sf = fold_all ? 1 : 0;
-            if (thr.is_const)
-              DISPATCH_SDFV(v, (k_extend_march<V, true><<<ctx->n_sm * ctx->occ_ext[1][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
-            else
-              DISPATCH_SDFV(v, (k_extend_march<V, false><<<ctx->n_sm * ctx->occ_ext[0][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
-            timed_end(ctx, RAYN_K_EXTEND);
-            ++e;
-          }
-          k = e;
-        }
+        if ((rc = extend_enqueue(ctx, P, pb, thr, resident(ctx->occ_sph)))) return rc;
       }
       timed_begin(ctx, RAYN_K_BIN);
       k_bin_count<<<dim3(nseg, nt), BIN_T, 0, st>>>(pb, n_hit, nseg);
@@ -1048,6 +1112,77 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* f, const R
   return render_finish(ctx);
 }
 
+// The first-hit albedo plane (statement in include/rayn_b200.h): the render's raygen and depth-0 closest-hit stage, then
+// k_albedo_paths and k_albedo_resolve (rt_albedo.cuh), pass by pass over the whole tile grid.  Never captured into a graph.
+int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float* albedo, int32_t space) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (ctx->pending) return fail(ctx, RAYN_ERR_INVALID_ARG, "a render is already in flight on this context");
+  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "render_albedo before upload_scene");
+  if (!f || !albedo) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/albedo is NULL");
+  if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_albedo: bad memory space %d", space);
+  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_albedo: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
+  FramePlan P;
+  int32_t rc = frame_check(ctx, f, true, &P);
+  if (rc) return rc;
+  DevFrame& fr = P.fr;
+  std::vector<int>& tiles = ctx->job_tiles;
+  tiles.clear();
+  for (int idx = 0; idx < fr.ntx * fr.nty; ++idx) tiles.push_back(idx);
+
+  memset(&ctx->stats, 0, sizeof ctx->stats);
+  ctx->timed_used = 0;
+  cudaStream_t st = ctx->stream;
+  if (f->input_space == RAYN_MEM_DEVICE || space == RAYN_MEM_DEVICE) CU(cudaDeviceSynchronize());
+  CU(cudaEventRecord(ctx->ev0, st));
+  if ((rc = upload_tables(ctx, f, &fr))) return rc;
+  const size_t npx = (size_t)f->width * f->height;
+  float* dst = albedo;
+  if (space == RAYN_MEM_HOST) {
+    CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 3));
+    dst = ctx->d_planes;
+  }
+  CU(cudaMemsetAsync(dst, 0, npx * 3 * sizeof(float), st));  // pixels outside the tile grid stay 0
+  if ((rc = scene_plan(ctx, &P))) return rc;
+  int tiles_per_pass;  // the render's own sizing: alternating renders and albedo passes reuse the same pass buffers
+  if ((rc = size_pass(ctx, P, tiles.size(), &tiles_per_pass))) return rc;
+  PassBufs pb = ctx->pb;
+  pb.R = P.R, pb.QS = P.QS, pb.tile_ids = ctx->d_tile_ids;
+  pb.lc_ns = P.lc_ns;
+  pb.seg_count = ctx->d_work_ctr + WC_SEG_COUNT;
+  CU(cudaMemsetAsync(pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), st));
+  const Thr thr = make_thr(ctx->scene.cam, 0);
+  for (size_t first = 0; first < tiles.size(); first += tiles_per_pass) {
+    const int nt = (int)std::min<size_t>(tiles_per_pass, tiles.size() - first);
+    pb.n_tiles = nt;
+    CU(cudaMemcpyAsync(ctx->d_tile_ids, tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, st));
+    ctx->stats.passes++;
+    const dim3 g_paths((P.R + 255) / 256, nt);
+    const int64_t max_blocks = (int64_t)nt * ((P.QS + SLOT_BLOCK - 1) / SLOT_BLOCK);
+    const unsigned sph_grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((int64_t)ctx->n_sm * ctx->occ_sph, max_blocks));
+    timed_begin(ctx, RAYN_K_RAYGEN);
+    k_raygen<<<g_paths, 256, 0, st>>>(ctx->scene, fr, pb, P.n_fold);
+    timed_end(ctx, RAYN_K_RAYGEN);
+    if ((rc = extend_enqueue(ctx, P, pb, thr, sph_grid))) return rc;
+    timed_begin(ctx, RAYN_K_NORMALS);
+    k_albedo_paths<<<g_paths, 256, 0, st>>>(ctx->scene, fr, pb, pb.nrm);
+    timed_end(ctx, RAYN_K_NORMALS);
+    timed_begin(ctx, RAYN_K_RESOLVE);
+    k_albedo_resolve<<<dim3((f->tile_w * f->tile_h + 255) / 256, nt), 256, 0, st>>>(fr, pb, pb.nrm, dst);
+    timed_end(ctx, RAYN_K_RESOLVE);
+    CU(cudaGetLastError());
+  }
+  ctx->job_w = f->width, ctx->job_h = f->height, ctx->job_tw = f->tile_w, ctx->job_th = f->tile_h, ctx->job_spp = fr.spp, ctx->job_nty = fr.nty;
+  ctx->pending = true;
+  if (space == RAYN_MEM_HOST) {
+    const cudaError_t e = cudaMemcpyAsync(albedo, dst, npx * 3 * sizeof(float), cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) {
+      render_finish(ctx);
+      CU(e);
+    }
+  }
+  return render_finish(ctx);
+}
+
 int32_t rayn_b200_sync(RaynContext* ctx) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   CU(cudaSetDevice(ctx->device));
@@ -1260,14 +1395,17 @@ static bool denoise_factor(float sigma, float* f) {
 
 // Enqueues the whole filter on ctx->stream.  `scratch` holds guide + ping-pong planes (12 floats per pixel), then the
 // device copies of host-space inputs (10) and one host-space output channel (3), as the caller sized it.
+// albedo != NULL (rayn_b200_film_denoise_albedo with a finite sigma): the albedo plane in in->space and its factor il; the
+// scratch then holds 4 more floats per pixel (its float4 guide) after the ping-pong planes, and 3 more for a host-space plane.
 static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W, int H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
-                               float ic0, float in_, float ia, float* scratch) {
+                               float ic0, float in_, float ia, float* scratch, const float* albedo = nullptr, float il = 0.0f) {
   cudaStream_t st = ctx->stream;
   const size_t npx = (size_t)W * H;
   const unsigned blocks1d = (unsigned)((npx + 255) / 256);
   float4* guide = (float4*)scratch;
   float4* ping[2] = {guide + npx, guide + 2 * npx};
-  float* stage = scratch + 12 * npx;
+  float4* alb = albedo ? guide + 3 * npx : nullptr;
+  float* stage = scratch + (albedo ? 16 : 12) * npx;
   const float *c_in = in->color, *b_in = in->background, *n_in = in->normal, *a_in = in->alpha;
   if (in->space == RAYN_MEM_HOST) {
     float* s = stage;
@@ -1279,6 +1417,15 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
     n_in = s, a_in = s + 3 * npx, c_in = in->color ? s + 4 * npx : nullptr, b_in = in->background ? s + 7 * npx : nullptr;
   }
   k_denoise_guides<<<blocks1d, 256, 0, st>>>((long long)npx, n_in, a_in, guide);
+  if (albedo) {
+    const float* l_in = albedo;
+    if (in->space == RAYN_MEM_HOST) {
+      CU(cudaMemcpyAsync(stage, albedo, npx * 12, cudaMemcpyHostToDevice, st));
+      l_in = stage;
+      stage += 3 * npx;
+    }
+    k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, l_in, alb);
+  }
   CU(cudaGetLastError());
   const dim3 blk(32, 8), grid((unsigned)((W + 31) / 32), (unsigned)((H + 7) / 8));
   for (int ch = 0; ch < 2; ++ch) {
@@ -1290,7 +1437,12 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
     for (int i = 0; i < d->iterations; ++i) {
       const float ic = ldexpf(ic0, i);
       const float4* src = ping[i & 1];
-      if (i == d->iterations - 1)
+      const bool last = i == d->iterations - 1;
+      if (albedo && last)
+        k_denoise_level<true, true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, nullptr, dst3, alb, il);
+      else if (albedo)
+        k_denoise_level<false, true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, ping[(i + 1) & 1], nullptr, alb, il);
+      else if (last)
         k_denoise_level<true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, nullptr, dst3);
       else
         k_denoise_level<false><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, ping[(i + 1) & 1], nullptr);
@@ -1301,8 +1453,9 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
   return RAYN_OK;
 }
 
-int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in,
-                               const RaynFilmPlanes* out) {
+// rayn_b200_film_denoise and, with an albedo plane (albedo != NULL), rayn_b200_film_denoise_albedo
+static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
+                            const float* albedo, float il) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!d || !in || !out || W <= 0 || H <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad argument");
   if (d->iterations < 1 || d->iterations > 8) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: iterations %d not in [1,8]", d->iterations);
@@ -1319,17 +1472,35 @@ int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32
   CU(cudaSetDevice(ctx->device));
   if (!in->color && !in->background) return RAYN_OK;
   const size_t npx = (size_t)W * H;
-  const size_t nfloat = npx * (12 + (in->space == RAYN_MEM_HOST ? 10 : 0) + (out->space == RAYN_MEM_HOST ? 3 : 0));
+  const size_t nfloat = npx * (12 + (in->space == RAYN_MEM_HOST ? 10 : 0) + (out->space == RAYN_MEM_HOST ? 3 : 0) +
+                               (albedo ? 4 + (in->space == RAYN_MEM_HOST ? 3 : 0) : 0));
   cudaStream_t st = ctx->stream;
   float* scratch = nullptr;
   // stream-ordered and released below: nothing persists between calls (render-pass sizing reads cudaMemGetInfo)
   CU(cudaMallocAsync((void**)&scratch, nfloat * sizeof(float), st));
-  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch);
+  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il);
   const cudaError_t ef = cudaFreeAsync(scratch, st);
   if (rc) return rc;
   CU(ef);
   if (in->space == RAYN_MEM_HOST || out->space == RAYN_MEM_HOST) CU(cudaStreamSynchronize(st));
   return RAYN_OK;
+}
+
+int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                               const RaynFilmPlanes* out) {
+  return film_denoise(ctx, d, W, H, in, out, nullptr, 0.0f);
+}
+
+int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_albedo, const float* albedo, int32_t W, int32_t H,
+                                      const RaynFilmPlanes* in, const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!albedo) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_albedo: the albedo plane is NULL");
+  float il;
+  if (!denoise_factor(sigma_albedo, &il))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_albedo: sigma_albedo %g must be > 0 (+inf disables the term) and give a finite 1/sigma^2",
+                sigma_albedo);
+  // +inf: the term is not added at all (adding dl2 * 0 would turn a non-finite albedo tap into a NaN tap)
+  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il);
 }
 
 int32_t rayn_b200_device_frame_inputs(RaynContext* ctx, int32_t W, int32_t H, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,

@@ -39,9 +39,12 @@ __global__ void __launch_bounds__(256) k_denoise_guides(long long npx, const flo
 }
 
 // One level with step 2^level.  kOut3: the last level writes the interleaved rgb output plane instead of a float4 plane.
-template <bool kOut3>
+// kAlb (rayn_b200_film_denoise_albedo): a fourth edge-stopping term dl2 * il from the albedo guide, packed (r, g, b, 0) by
+// k_denoise_pack; the kAlb = false instances never read `alb` or `il` and run the code of rayn_b200_film_denoise.
+template <bool kOut3, bool kAlb = false>
 __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, float ic, float in_, float ia, const float4* __restrict__ guide,
-                                                       const float4* __restrict__ src, float4* __restrict__ dst4, float* __restrict__ dst3) {
+                                                       const float4* __restrict__ src, float4* __restrict__ dst4, float* __restrict__ dst3,
+                                                       const float4* __restrict__ alb = nullptr, float il = 0.0f) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= W || y >= H) return;
   const size_t p = (size_t)y * W + x;
@@ -50,6 +53,7 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
   if (dn_finite3(cp)) {
     const float h[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
     const float4 gp = guide[p];
+    const float4 lp = kAlb ? alb[p] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     float sr = 0.0f, sg = 0.0f, sb = 0.0f, sw = 0.0f;
 #pragma unroll
     for (int dy = -2; dy <= 2; ++dy) {
@@ -70,7 +74,17 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
         const float dn2 = (nx * nx + ny * ny) + nz * nz;
         const float da = gq.w - gp.w;
         const float da2 = da * da;
-        const float e = (dc2 * ic + dn2 * in_) + da2 * ia;
+        float e = (dc2 * ic + dn2 * in_) + da2 * ia;
+        if (kAlb) {
+          // Every term of e is a product of a square (>= 0 or NaN) and a factor >= 0, so e is still a sum of non-negative
+          // terms or NaN (0 * inf = NaN cannot occur: every factor is finite).  Hence both shortcuts hold unchanged: e == 0
+          // still means exp(-e) = 1 exactly, and e > DENOISE_E_DEAD or NaN still means a skipped tap.  A non-finite albedo
+          // component makes dl2 NaN or +inf, i.e. a NaN tap (skipped) or a dead one (weight +0), as in the statement.
+          const float4 lq = alb[(size_t)qy * W + qx];
+          const float ar = lq.x - lp.x, ag = lq.y - lp.y, ab = lq.z - lp.z;
+          const float dl2 = (ar * ar + ag * ag) + ab * ab;
+          e = e + dl2 * il;
+        }
         if (!(e <= DENOISE_E_DEAD)) continue;  // NaN (skipped by the statement) or a weight of exactly +0 (argument above)
         const float hk = h[dy + 2] * h[dx + 2];
         const float w = e == 0.0f ? hk : hk * dm::exp(-e);

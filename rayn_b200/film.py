@@ -17,6 +17,8 @@ from . import _lib as L
 from .scene import BlackmanHarrisFilter, PathTracingIntegrator
 
 CHANNELS = ("color", "alpha", "background", "normal")  # ChannelKind, film.rs:103-120
+# a Film may also hold the first-hit albedo plane (Renderer.render_albedo), which the reference has no channel for
+FILM_CHANNELS = CHANNELS + ("albedo",)
 
 
 def _fptr(a):
@@ -72,6 +74,13 @@ def make_frame_desc(width, height, tile_size, samples, integrator, frame, time_r
 # Picked by `tools/bench_denoise.py --pick-sigmas` (DESIGN.md §4b): the lowest col+bg MSE against a 256 spp film of a
 # 4 spp config 3 film at 96x96, 5 levels, over a grid of 9 x 6 x 4 sigmas.
 DENOISE_DEFAULTS = dict(sigma_color=2.5, sigma_normal=0.4, sigma_alpha=0.5)
+
+
+# The albedo-guided filter (rayn_b200_film_denoise_albedo) and the albedo plane of a Film: picked by `tools/bench_albedo.py`
+# (DESIGN.md §4e) on config 3 with the README palette at 96x96.  ALBEDO_SAMPLES caps the plane's samples (4 * ALBEDO_SAMPLES
+# spp, the first camera samples of the film's own sequences): first-hit albedo converges much faster than colour.
+DENOISE_ALBEDO_SIGMA = 0.2
+ALBEDO_SAMPLES = 16
 
 
 def denoise_desc(iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
@@ -192,6 +201,17 @@ class Renderer:
         self.render(f, p)
         return planes
 
+    def render_albedo(self, inputs, tile_size, integrator, time_range):
+        """First-hit albedo plane of the uploaded scene (include/rayn_b200.h: rayn_b200_render_albedo) for host FrameInputs:
+        float32 [H, W, 3]."""
+        w, h = inputs.width, inputs.height
+        out = np.zeros(3 * w * h, np.float32)
+        ptrs = tuple(a.ctypes.data for a in inputs.arrays())
+        f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST,
+                            sets=(inputs.sets_1d, inputs.sets_2d))
+        L.check(self._lib.rayn_b200_render_albedo(self._ctx, C.byref(f), out.ctypes.data, L.MEM_HOST), self._ctx)
+        return out.reshape(h, w, 3)
+
     def postprocess(self, mode, width, height, planes):
         """Film::save_to pixel arithmetic on the device (film.rs:205-377): numpy planes in, uint8 [H, W, bpp] out (rows top to bottom)."""
         def ptr(k):
@@ -201,10 +221,13 @@ class Renderer:
         L.check(self._lib.rayn_b200_film_postprocess(self._ctx, mode, width, height, C.byref(p), out.ctypes.data, L.MEM_HOST), self._ctx)
         return out
 
-    def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
+    def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, albedo=None,
+                sigma_albedo=None):
         """Edge-avoiding a-trous filter of the color and background planes (include/rayn_b200.h: rayn_b200_film_denoise).
         numpy planes in ("normal" and "alpha" required, "color" / "background" optional); returns new arrays for the
-        colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term."""
+        colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term.
+        albedo (a [3*W*H] plane, e.g. render_albedo's): the albedo-guided filter (rayn_b200_film_denoise_albedo) with
+        sigma_albedo, default DENOISE_ALBEDO_SIGMA."""
         for k in ("normal", "alpha"):
             if planes.get(k) is None:
                 raise ValueError(f"denoise needs the {k} guide plane")
@@ -216,7 +239,13 @@ class Renderer:
         pin = L.RaynFilmPlanes(ptr(flat, "color"), ptr(flat, "alpha"), ptr(flat, "background"), ptr(flat, "normal"), L.MEM_HOST)
         pout = L.RaynFilmPlanes(ptr(outs, "color"), None, ptr(outs, "background"), None, L.MEM_HOST)
         desc = denoise_desc(iterations, sigma_color, sigma_normal, sigma_alpha)
-        L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
+        if albedo is None:
+            L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
+        else:
+            alb = np.ascontiguousarray(albedo, np.float32).reshape(-1)
+            sa = float(DENOISE_ALBEDO_SIGMA if sigma_albedo is None else sigma_albedo)
+            L.check(self._lib.rayn_b200_film_denoise_albedo(self._ctx, C.byref(desc), sa, alb.ctypes.data, width, height, C.byref(pin),
+                                                            C.byref(pout)), self._ctx)
         return {k: v.reshape(np.shape(planes[k])) for k, v in outs.items()}
 
     # ---- progressive / adaptive rendering (rayn_b200_accum_*) ----
@@ -352,7 +381,7 @@ class Film:
         if len(set(channels)) != len(channels):
             raise ValueError("Attempted to create multiple channels of one kind")  # film.rs:187-189
         for c in channels:
-            if c not in CHANNELS:
+            if c not in FILM_CHANNELS:
                 raise ValueError(f"unknown channel {c}")
         self.channel_kinds = tuple(channels)
         self.res = (int(res[0]), int(res[1]))
@@ -372,8 +401,19 @@ class Film:
         planes = self._renderer.render_host(inputs, tile_size, integrator, time_range)
         self.last_stats = self._renderer.stats()
         for k in self.channel_kinds:
-            self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
+            if k != "albedo":
+                self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
+        self._render_albedo(integrator, filt, tile_size, frame, time_range, samples)
         self.progressive_epoch += 1  # film.rs:657
+
+    def _render_albedo(self, integrator, filt, tile_size, frame, time_range, samples):
+        """Fills the "albedo" channel, if the Film has one: one render_albedo call with the frame's seed and the first
+        4 * min(samples, ALBEDO_SAMPLES) camera samples of its sequences."""
+        if "albedo" not in self.channel_kinds:
+            return
+        w, h = self.res
+        inputs = FrameInputs(w, h, min(samples, ALBEDO_SAMPLES), integrator, filt, frame)
+        self.channels["albedo"] = self._renderer.render_albedo(inputs, tile_size, integrator, time_range)
 
     def render_adaptive(self, world, camera, integrator, filt, tile_size, frame, time_range, samples_per_round, min_rounds=2,
                         max_rounds=ADAPTIVE_MAX_ROUNDS, threshold=ADAPTIVE_THRESHOLD, on_round=None):
@@ -420,13 +460,15 @@ class Film:
                 self._take_accum(r, acc)
         finally:
             acc.close()
+        self._render_albedo(integrator, filt, tile_size, frame, time_range, samples_per_round * max_rounds)
         return rounds
 
     def _take_accum(self, r, acc):
         w, h = self.res
         planes = r.accum_resolve(acc)
         for k in self.channel_kinds:
-            self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
+            if k != "albedo":
+                self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
         self.tile_errors, self.tile_samples = r.accum_tiles(acc)
         self.progressive_epoch += 1  # film.rs:657
 
@@ -449,28 +491,35 @@ class Film:
                     mode, pil = L.POST_COLOR_ONLY, "RGB"
                 else:
                     raise ValueError("Attempted to write Color channel with insufficient channels")  # film.rs:294-298
-            elif kind in ("background", "normal", "alpha"):
+            elif kind in ("background", "normal", "alpha", "albedo"):
                 if kind not in flat:
                     raise ValueError(f"Attempted to write {kind} channel but it didn't exist")
-                mode, pil = {"background": (L.POST_BACKGROUND, "RGB"), "normal": (L.POST_WORLD_NORMAL, "RGB"), "alpha": (L.POST_ALPHA, "L")}[kind]
+                mode, pil = {"background": (L.POST_BACKGROUND, "RGB"), "normal": (L.POST_WORLD_NORMAL, "RGB"), "alpha": (L.POST_ALPHA, "L"),
+                             "albedo": (L.POST_BACKGROUND, "RGB")}[kind]
             else:
                 raise ValueError(kind)
-            px = self._renderer.postprocess(mode, w, h, flat)
+            # the albedo plane is written with the background's arithmetic (saturate, gamma 2.2)
+            px = self._renderer.postprocess(mode, w, h, {"background": flat["albedo"]} if kind == "albedo" else flat)
             path = os.path.join(output_folder, f"{base_name}_{kind}.png")
             Image.fromarray(px[:, :, 0] if pil == "L" else px, pil).save(path)
             written.append(path)
         return written
 
-    def denoise(self, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
+    def denoise(self, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, sigma_albedo=None):
         """Filters the Film's color and background channels in place (Renderer.denoise), guided by its normal and alpha
-        channels.  Call it after render_frame_into and before save_to."""
+        channels, and by its albedo channel if it has one (sigma_albedo, default DENOISE_ALBEDO_SIGMA).  Call it after
+        render_frame_into and before save_to."""
         for k in ("normal", "alpha"):
             if k not in self.channels:
                 raise ValueError(f"Film.denoise needs the {k} channel")
         if self._renderer is None:
             self._renderer = Renderer(self._device)
         w, h = self.res
-        self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha))
+        if "albedo" in self.channels:
+            self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha,
+                                                        albedo=self.channels["albedo"], sigma_albedo=sigma_albedo))
+        else:
+            self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha))
 
     def tonemapped_rgb8(self):
         """The display formula of save_to (film.rs:253-267): (color + background).saturated().gamma(2.2), y flipped."""

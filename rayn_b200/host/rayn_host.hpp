@@ -326,15 +326,38 @@ class Film {
     rayn_b200_accum_destroy(acc);
     return rounds;
   }
+  // First-hit albedo plane of the frame (rayn_b200_render_albedo) into `albedo`: the first 4*samples camera samples of the
+  // frame's sequences.
+  void render_albedo(const World& world, CameraHandle camera, const PathTracingIntegrator& integrator, const BlackmanHarrisFilter& filter,
+                     int tile_w, int tile_h, int frame, float t0, float t1, int samples) {
+    const int spp = 4 * samples;
+    const int sets_1d = 1 + integrator.requested_1d_sample_sets(), sets_2d = 2 + integrator.requested_2d_sample_sets();
+    std::vector<float> s1((size_t)spp * sets_1d), s2((size_t)2 * spp * sets_2d), scr((size_t)w_ * h_), fis(RAYN_FIS_TABLE_SIZE);
+    check(rayn_b200_host_rd_tables(spp, sets_1d, sets_2d, (uint64_t)frame, s1.data(), s2.data()), ctx_);
+    check(rayn_b200_host_scramble(w_, h_, scr.data()), ctx_);
+    check(rayn_b200_host_fis_blackman_harris(filter.radius, fis.data()), ctx_);
+    upload_scene(world, camera);
+    RaynFrameDesc f = frame_desc(integrator, tile_w, tile_h, frame, t0, t1, samples, sets_1d, sets_2d);
+    f.samples_1d = s1.data(), f.samples_2d = s2.data(), f.scramble = scr.data(), f.fis_inverse_cdf = fis.data();
+    albedo.assign((size_t)3 * w_ * h_, 0.0f);
+    check(rayn_b200_render_albedo(ctx_, &f, albedo.data(), RAYN_MEM_HOST), ctx_);
+  }
   // Edge-avoiding a-trous filter of color and background in place, guided by normal and alpha (rayn_b200_film_denoise).
   void denoise(int iterations, float sigma_color, float sigma_normal, float sigma_alpha) {
     const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
     RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
     check(rayn_b200_film_denoise(ctx_, &d, w_, h_, &p, &p), ctx_);
   }
+  // ... also guided by the albedo plane of render_albedo (rayn_b200_film_denoise_albedo)
+  void denoise_albedo(int iterations, float sigma_color, float sigma_normal, float sigma_alpha, float sigma_albedo) {
+    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    check(rayn_b200_film_denoise_albedo(ctx_, &d, sigma_albedo, albedo.data(), w_, h_, &p, &p), ctx_);
+  }
   int width() const { return w_; }
   int height() const { return h_; }
   std::vector<float> color, alpha, background, normal;
+  std::vector<float> albedo;          // render_albedo: [3*W*H]
   std::vector<double> tile_errors;    // render_adaptive: E per tile index tile_x * n_tiles_y + tile_y
   std::vector<int64_t> tile_samples;  // ... and samples per pixel
   RaynStats stats{};
