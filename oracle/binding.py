@@ -66,13 +66,10 @@ def _f(a):
 def render(world, camera, inputs, tile_size, integrator, time_range, n_threads=0, subsample_k=1, tile_offset=0, tile_stride=1,
            queue_log=False, tile_list=None):
     """CPU render of the same FrameInputs.  Returns (planes dict, info dict)."""
-    from rayn_b200.film import make_frame_desc
+    from rayn_b200.film import host_planes, make_frame_desc
     desc, keep = world.flatten(camera)
     w, h = inputs.width, inputs.height
-    planes = {"color": np.zeros(3 * w * h, np.float32), "alpha": np.zeros(w * h, np.float32),
-              "background": np.zeros(3 * w * h, np.float32), "normal": np.zeros(3 * w * h, np.float32)}
-    p = L.RaynFilmPlanes(planes["color"].ctypes.data, planes["alpha"].ctypes.data, planes["background"].ctypes.data,
-                         planes["normal"].ctypes.data, L.MEM_HOST)
+    planes, p = host_planes(w, h)
     ptrs = tuple(a.ctypes.data for a in inputs.arrays())
     f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST, tile_offset,
                         tile_stride, (inputs.sets_1d, inputs.sets_2d), tile_list)

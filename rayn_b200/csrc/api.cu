@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <string>
 #include <vector>
 
@@ -57,6 +58,14 @@ struct RaynComm {
   size_t cap_slabs = 0;
 };
 
+// One entry of the pass-buffer table (pass_table): a buffer and its size in bytes, per_path * paths + per_slot * shading
+// slots + per_tile * tiles + fixed.  An entry whose size is 0 (its condition does not hold) is not allocated.
+struct PassBuf {
+  void** ptr;
+  size_t per_path, per_slot, per_tile, fixed;
+};
+static const int N_PASS_BUFS = 23;
+
 struct RaynContext {
   int device = 0;
   int flags = 0;
@@ -66,15 +75,10 @@ struct RaynContext {
   DevScene scene;
   int64_t cap_paths = 0;  // requested paths per pass
   // pass buffers
-  int64_t alloc_paths = 0, alloc_q = 0, alloc_seg = 0;
-  int alloc_lc_ns = 0;
-  bool alloc_trap = false;  // PassBufs::trap_s is allocated
-  int alloc_tiles = 0;
-  int64_t alloc_segcnt = 0;  // ints in PassBufs::seg_cnt
-  size_t pass_bytes = 0;
+  size_t pass_cap[N_PASS_BUFS] = {};  // bytes allocated per pass_table entry
   PassBufs pb;
   int* d_tile_ids = nullptr;
-  int* d_batch_prefix = nullptr;  // [alloc_tiles + 1]
+  int* d_batch_prefix = nullptr;  // [tiles per pass + 1]
   int* d_work_ctr = nullptr;      // [WC_TOTAL] global work counters of the persistent kernels
   int n_sm = 148;
   int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT], occ_nrm_trap[SDFV_COUNT];  // occ_ext[constant threshold][variant]
@@ -156,92 +160,83 @@ static cudaError_t regrow(T** p, size_t* cap, size_t need) {
   return e;
 }
 
-static void free_pass(RaynContext* c) {
+// Every pass buffer, in allocation order.  seg_per_path: shadow segments per path and depth over all SDF queues; lc_ns: light
+// samples per path and depth; trap: the scene has orbit-trap albedos (PassBufs::trap_s).
+static std::array<PassBuf, N_PASS_BUFS> pass_table(RaynContext* c, int QS, int seg_per_path, int lc_ns, bool trap) {
   PassBufs& p = c->pb;
-  cudaFree(p.o_time), cudaFree(p.d_t), cudaFree(p.rad), cudaFree(p.thr), cudaFree(p.nrm0), cudaFree(p.term);
-  cudaFree(p.q_live), cudaFree(p.q_key), cudaFree(p.q_shade), cudaFree(p.n_live), cudaFree(p.n_slots), cudaFree(p.bin_start);
-  cudaFree(c->d_tile_ids);
-  cudaFree(c->d_batch_prefix);
-  c->d_batch_prefix = nullptr;
-  cudaFree(p.nrm), cudaFree(p.vis), cudaFree(p.seg_a), cudaFree(p.seg_b), cudaFree(p.lc_c), cudaFree(p.lc_t), cudaFree(p.seg_cnt), cudaFree(p.slot_prefix);
-  cudaFree(p.trap_s);
-  unsigned long long* counters = p.counters;
-  memset(&p, 0, sizeof p);
-  p.counters = counters;
-  c->d_tile_ids = nullptr;
-  c->alloc_paths = c->alloc_q = c->alloc_seg = 0;
-  c->alloc_lc_ns = 0;
-  c->alloc_trap = false;
-  c->alloc_tiles = 0;
-  c->alloc_segcnt = 0;
-  c->pass_bytes = 0;
+  const size_t nseg = (QS + SEG_SLOTS - 1) / SEG_SLOTS;  // segments per tile of the queue kernels
+  return {{
+      {(void**)&p.o_time, sizeof(float4), 0, 0, 0},
+      {(void**)&p.d_t, sizeof(float4), 0, 0, 0},
+      {(void**)&p.rad, sizeof(float4), 0, 0, 0},
+      {(void**)&p.thr, sizeof(float4), 0, 0, 0},
+      {(void**)&p.nrm0, sizeof(float4), 0, 0, 0},
+      {(void**)&p.term, sizeof(uint32_t), 0, 0, 0},
+      {(void**)&p.q_live, sizeof(int), 0, 0, 0},
+      {(void**)&p.q_key, sizeof(int), 0, 0, 0},
+      {(void**)&p.q_shade, 0, sizeof(int), 0, 0},
+      {(void**)&p.n_live, 0, 0, sizeof(int), 0},
+      {(void**)&p.n_slots, 0, 0, sizeof(int), 0},
+      {(void**)&p.bin_start, 0, 0, (RAYN_MAX_HITABLES + 1) * sizeof(int), 0},
+      {(void**)&c->d_tile_ids, 0, 0, sizeof(int), 0},
+      {(void**)&c->d_batch_prefix, 0, 0, sizeof(int), sizeof(int)},
+      {(void**)&p.seg_cnt, 0, 0, nseg * RAYN_MAX_HITABLES * sizeof(int), 0},
+      {(void**)&p.slot_prefix, 0, 0, (1 + RAYN_MAX_HITABLES) * sizeof(int), (1 + RAYN_MAX_HITABLES) * sizeof(int)},
+      {(void**)&p.nrm, sizeof(float4), 0, 0, 0},
+      {(void**)&p.vis, sizeof(uint32_t), 0, 0, 0},
+      {(void**)&p.seg_a, (size_t)seg_per_path * sizeof(float4), 0, 0, 0},
+      {(void**)&p.seg_b, (size_t)seg_per_path * sizeof(float4), 0, 0, 0},
+      {(void**)&p.lc_c, (size_t)lc_ns * sizeof(float4), 0, 0, 0},
+      {(void**)&p.lc_t, lc_ns > 4 ? 8 * sizeof(float) : 0, 0, 0, 0},
+      {(void**)&p.trap_s, trap ? sizeof(float) : 0, 0, 0, 0},
+  }};
 }
 
-// bytes of pass state per path (what ensure_pass allocates), used to size passes against free device memory
-static size_t pass_bytes_per_path(int R, int QS, int seg_per_path, int lc_ns, bool trap) {
-  return 6 * sizeof(float4) + 2 * sizeof(uint32_t) + 2 * sizeof(int) + (size_t)(((double)QS / R) * sizeof(int) + 1) + (size_t)lc_ns * sizeof(float4) +
-         (lc_ns > 4 ? 8 * sizeof(float) : 0) + (size_t)seg_per_path * 2 * sizeof(float4) + (trap ? sizeof(float) : 0);
+static void free_pass(RaynContext* c) {
+  for (const PassBuf& b : pass_table(c, 0, 0, 0, false)) {
+    cudaFree(*b.ptr);
+    *b.ptr = nullptr;
+  }
+  unsigned long long* counters = c->pb.counters;
+  memset(&c->pb, 0, sizeof c->pb);
+  c->pb.counters = counters;
+  memset(c->pass_cap, 0, sizeof c->pass_cap);
 }
 
-// trap: the scene has orbit-trap albedos, so the per-path palette coordinate PassBufs::trap_s is needed as well
-static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg_per_path_total, int n_sdf, int lc_ns, bool trap) {
+// bytes of pass state per path (what ensure_pass allocates, less the per-tile buffers), used to size passes against free
+// device memory
+static size_t pass_bytes_per_path(RaynContext* c, int R, int QS, int seg_per_path, int lc_ns, bool trap) {
+  size_t bytes = 0;
+  for (const PassBuf& b : pass_table(c, QS, seg_per_path, lc_ns, trap))
+    bytes += b.per_path + (b.per_slot ? (size_t)(((double)QS / R) * b.per_slot + 1) : 0);
+  return bytes;
+}
+
+static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg_per_path, int n_sdf, int lc_ns, bool trap) {
   const int64_t need_paths = (int64_t)n_tiles * R, need_q = (int64_t)n_tiles * QS;
-  const int64_t need_seg = need_paths * seg_per_path_total;  // all SDF queues together
-  const int64_t need_segcnt = (int64_t)n_tiles * ((QS + SEG_SLOTS - 1) / SEG_SLOTS) * RAYN_MAX_HITABLES;
-  if (need_paths <= ctx->alloc_paths && need_q <= ctx->alloc_q && n_tiles <= ctx->alloc_tiles && need_seg <= ctx->alloc_seg && lc_ns <= ctx->alloc_lc_ns &&
-      need_segcnt <= ctx->alloc_segcnt && (!trap || ctx->alloc_trap))
-    return RAYN_OK;
+  const std::array<PassBuf, N_PASS_BUFS> table = pass_table(ctx, QS, seg_per_path, lc_ns, trap);
+  size_t need[N_PASS_BUFS];
+  bool fits = true;
+  for (int i = 0; i < N_PASS_BUFS; ++i) {
+    const PassBuf& b = table[i];
+    need[i] = b.per_path * need_paths + b.per_slot * need_q + b.per_tile * n_tiles + b.fixed;
+    fits = fits && need[i] <= ctx->pass_cap[i];
+  }
+  if (fits) return RAYN_OK;
   free_pass(ctx);
-  PassBufs& p = ctx->pb;
-  size_t total = 0;
-#define PASS_ALLOC(ptr, bytes)                                    \
-  do {                                                            \
-    cudaError_t e_ = cudaMalloc((void**)&(ptr), (size_t)(bytes)); \
-    if (e_ != cudaSuccess) {                                      \
-      cudaGetLastError();                                         \
-      free_pass(ctx);                                             \
-      return fail(ctx, e_ == cudaErrorMemoryAllocation ? RAYN_ERR_OOM : RAYN_ERR_CUDA, "pass buffers (%lld paths): %s", (long long)need_paths, cudaGetErrorString(e_)); \
-    }                                                             \
-    total += (size_t)(bytes);                                     \
-  } while (0)
-  PASS_ALLOC(p.o_time, need_paths * sizeof(float4));
-  PASS_ALLOC(p.d_t, need_paths * sizeof(float4));
-  PASS_ALLOC(p.rad, need_paths * sizeof(float4));
-  PASS_ALLOC(p.thr, need_paths * sizeof(float4));
-  PASS_ALLOC(p.nrm0, need_paths * sizeof(float4));
-  PASS_ALLOC(p.term, need_paths * sizeof(uint32_t));
-  PASS_ALLOC(p.q_live, need_paths * sizeof(int));
-  PASS_ALLOC(p.q_key, need_paths * sizeof(int));
-  PASS_ALLOC(p.q_shade, need_q * sizeof(int));
-  PASS_ALLOC(p.n_live, n_tiles * sizeof(int));
-  PASS_ALLOC(p.n_slots, n_tiles * sizeof(int));
-  PASS_ALLOC(p.bin_start, (size_t)n_tiles * (RAYN_MAX_HITABLES + 1) * sizeof(int));
-  PASS_ALLOC(ctx->d_tile_ids, n_tiles * sizeof(int));
-  PASS_ALLOC(ctx->d_batch_prefix, ((size_t)n_tiles + 1) * sizeof(int));
-  PASS_ALLOC(p.seg_cnt, need_segcnt * sizeof(int));
-  PASS_ALLOC(p.slot_prefix, (size_t)(1 + RAYN_MAX_HITABLES) * ((size_t)n_tiles + 1) * sizeof(int));
-  p.prefix_stride = n_tiles + 1;
-  ctx->alloc_segcnt = need_segcnt;
-  PASS_ALLOC(p.nrm, need_paths * sizeof(float4));
-  PASS_ALLOC(p.vis, need_paths * sizeof(uint32_t));
-  if (need_seg > 0) {
-    PASS_ALLOC(p.seg_a, need_seg * sizeof(float4));
-    PASS_ALLOC(p.seg_b, need_seg * sizeof(float4));
+  for (int i = 0; i < N_PASS_BUFS; ++i) {
+    if (need[i] == 0) continue;
+    const cudaError_t e = cudaMalloc(table[i].ptr, need[i]);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      free_pass(ctx);
+      return fail(ctx, e == cudaErrorMemoryAllocation ? RAYN_ERR_OOM : RAYN_ERR_CUDA, "pass buffers (%lld paths): %s", (long long)need_paths,
+                  cudaGetErrorString(e));
+    }
+    ctx->pass_cap[i] = need[i];
   }
-  p.seg_cap = n_sdf > 0 ? need_seg / n_sdf : 0;
-  ctx->alloc_seg = need_seg;
-  if (lc_ns > 0) {
-    PASS_ALLOC(p.lc_c, need_paths * lc_ns * sizeof(float4));
-    if (lc_ns > 4) PASS_ALLOC(p.lc_t, need_paths * 8 * sizeof(float));
-  }
-  if (trap) PASS_ALLOC(p.trap_s, need_paths * sizeof(float));
-#undef PASS_ALLOC
-  ctx->alloc_trap = trap;
-  ctx->alloc_lc_ns = lc_ns;
-  ctx->alloc_paths = need_paths;
-  ctx->alloc_q = need_q;
-  ctx->alloc_tiles = n_tiles;
-  ctx->pass_bytes = total;
+  ctx->pb.prefix_stride = n_tiles + 1;
+  ctx->pb.seg_cap = n_sdf > 0 ? need_paths * seg_per_path / n_sdf : 0;
   return RAYN_OK;
 }
 
@@ -557,10 +552,24 @@ int64_t rayn_b200_debug_read_queue_log(RaynContext* ctx, int32_t* out, int64_t c
 struct FramePlan {
   DevFrame fr;
   int R, QS, np, wpc;  // paths and shading slots per tile; k_resolve's padded spp and warps per CTA
-  int n_sdf, sdf_idx[RAYN_MAX_HITABLES];
-  bool simple, motion, traps, fold_all, volume_on;
+  bool simple, traps, fold_all, volume_on;
   int fold_pre, n_fold, ns, seg_per_path, lc_ns;
 };
+
+// One render or albedo pass on a context: its plan and pass size (job_begin) and the pass being enqueued (pass_tiles).  The
+// job's tiles are ctx->job_tiles.
+struct Job {
+  FramePlan P;
+  PassBufs pb;  // pb.n_tiles: the tiles of the current pass
+  int tiles_per_pass;
+};
+
+// The resident grid (one wave) of a kernel that strides over a work list of the pass (k_scan_slots / k_scan_live), capped
+// by the list's upper bound.
+static unsigned resident(const RaynContext* ctx, const Job& J, int occ) {
+  const int64_t max_blocks = (int64_t)J.pb.n_tiles * ((J.P.QS + SLOT_BLOCK - 1) / SLOT_BLOCK);
+  return (unsigned)std::max<int64_t>(1, std::min<int64_t>((int64_t)ctx->n_sm * occ, max_blocks));
+}
 
 // The frame checks of render_frame and the DevFrame of the frame (tables not uploaded yet).  tiles_given: the caller picks
 // the tiles itself, so tile_offset / tile_stride are not checked.
@@ -631,18 +640,10 @@ static int32_t upload_tables(RaynContext* ctx, const RaynFrameDesc* f, DevFrame*
 
 // Which kernels the scene needs and how the closest-hit fold is split between them.
 static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
-  const int n_hit = ctx->scene.n_hit, vm = P->fr.vm;
-  int& n_sdf = P->n_sdf;
-  int* sdf_idx = P->sdf_idx;
-  n_sdf = 0;
-  for (int i = 0; i < n_hit; ++i)
-    if (ctx->scene.hit[i].kind != RAYN_HITABLE_SPHERE) sdf_idx[n_sdf++] = i;
+  const int n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, vm = P->fr.vm;
   const bool simple = P->simple = (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) != 0;
-  bool& motion = P->motion;
-  motion = false;  // time-varying sphere centres need the packet's lane-0 time: only the product kernels plumb it
-  for (int i = 0; i < n_hit; ++i)
-    motion |= ctx->scene.hit[i].kind == RAYN_HITABLE_SPHERE && (ctx->scene.hit[i].center_velocity[0] != 0.0f || ctx->scene.hit[i].center_velocity[1] != 0.0f ||
-                                                                 ctx->scene.hit[i].center_velocity[2] != 0.0f);
+  // time-varying sphere centres need the packet's lane-0 time: only the product kernels plumb it
+  const bool motion = ctx->scene.sph_moving != 0;
   if (motion && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "time-varying sphere centres are not supported by the legacy test kernels");
   const bool traps = P->traps = ctx->scene.trap_mask != 0u;
   if (traps && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "orbit-trap albedos are not supported by the legacy test kernels");
@@ -659,7 +660,7 @@ static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
   // launch) and shorter marches for rays that end on an emitter.  The result is the reference's fold bit for bit
   // (proof in rt_kernels.cuh at k_extend_march: it needs a distance estimator that is never negative, i.e. the Mandelbox -
   // sqrt(m) / |dr| - so that a march's t never decreases, and the first-index-wins tie rule, which the kernel applies).
-  const bool fold_all = P->fold_all = fold_pre >= 0 && n_sdf == 1 && ctx->scene.hit[sdf_idx[0]].kind == RAYN_HITABLE_MANDELBOX && !(ctx->flags & RAYN_FLAG_NO_FOLD_ALL);
+  const bool fold_all = P->fold_all = fold_pre >= 0 && n_sdf == 1 && ctx->scene.hit[ctx->scene.sdf_idx[0]].kind == RAYN_HITABLE_MANDELBOX && !(ctx->flags & RAYN_FLAG_NO_FOLD_ALL);
   P->n_fold = fold_all ? ctx->scene.n_sph : fold_pre;  // leading spheres are the first fold_pre entries of the compact sphere list
   const bool volume_on = P->volume_on = ctx->scene.vol.has_scattering != 0 && ctx->scene.n_lights > 0;
   const int ns = P->ns = volume_on ? 4 * (1 + vm) : 4;               // light samples per path per depth
@@ -670,12 +671,13 @@ static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
 
 // Pass size for n_tiles tiles (as many tiles per pass as the path budget and free device memory allow), and the pass buffers.
 static int32_t size_pass(RaynContext* ctx, const FramePlan& P, size_t n_tiles, int* out_tiles_per_pass) {
-  const int R = P.R, QS = P.QS, n_sdf = P.n_sdf, ns = P.ns, seg_per_path = P.seg_per_path, lc_ns = P.lc_ns;
+  const int R = P.R, QS = P.QS, n_sdf = ctx->scene.n_sdf, ns = P.ns, seg_per_path = P.seg_per_path, lc_ns = P.lc_ns;
   const bool traps = P.traps;
-  const size_t bpp = pass_bytes_per_path(R, QS, seg_per_path, lc_ns, traps);
-  size_t free_b = 0, total_b = 0;
+  const size_t bpp = pass_bytes_per_path(ctx, R, QS, seg_per_path, lc_ns, traps);
+  size_t free_b = 0, total_b = 0, pass_bytes = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
-  const size_t budget = (size_t)((double)(free_b + ctx->pass_bytes) * 0.90);
+  for (size_t b : ctx->pass_cap) pass_bytes += b;
+  const size_t budget = (size_t)((double)(free_b + pass_bytes) * 0.90);
   int64_t max_paths = std::min<int64_t>(ctx->cap_paths, (int64_t)(budget / bpp));
   if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, ((int64_t)1 << 27) - 1);          // owner path index is packed with the sample bit (<< 4)
   if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, (int64_t)INT_MAX / std::max(ns, 1));  // 32-bit queue cursors per SDF
@@ -690,11 +692,12 @@ static int32_t size_pass(RaynContext* ctx, const FramePlan& P, size_t n_tiles, i
 }
 
 // One depth's closest-hit stage (the non-legacy kernels): k_scan_live, then the fold over the live rays of the pass.
-// sph_grid: the resident grid of k_extend_spheres.
-static int32_t extend_enqueue(RaynContext* ctx, const FramePlan& P, const PassBufs& pb, const Thr& thr, unsigned sph_grid) {
+static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
   cudaStream_t st = ctx->stream;
-  const int n_hit = ctx->scene.n_hit, fold_pre = P.fold_pre;
-  const bool fold_all = P.fold_all, motion = P.motion;
+  const PassBufs& pb = J.pb;
+  const int n_hit = ctx->scene.n_hit, fold_pre = J.P.fold_pre;
+  const bool fold_all = J.P.fold_all, motion = ctx->scene.sph_moving != 0;
+  const unsigned sph_grid = resident(ctx, J, ctx->occ_sph);
   timed_begin(ctx, RAYN_K_MISC);
   k_scan_live<<<1, SCAN_T, 0, st>>>(pb, ctx->d_batch_prefix, ctx->d_work_ctr);
   timed_end(ctx, RAYN_K_MISC);
@@ -727,25 +730,32 @@ static int32_t extend_enqueue(RaynContext* ctx, const FramePlan& P, const PassBu
   return RAYN_OK;
 }
 
-// Enqueues one render on the context's stream.  Nothing here waits for the GPU (except the debug queue log), so a single
-// host thread can keep several GPUs busy (render_frame_multi).  tiles_override replaces the frame's own tile selection.
-// dev_planes_out (optional) receives the device-space planes the film was rendered into.
-static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
-                              RaynFilmPlanes* dev_planes_out) {
+// ---- the job driver of a render (render_enqueue) and an albedo pass (rayn_b200_render_albedo) ---------------------------
+// job_ready and job_begin, then per pass pass_tiles, pass_raygen and the job's own kernels; the job is then pending.
+
+// The context checks of every job, made before the call's own argument checks.
+static int32_t job_ready(RaynContext* ctx, const char* call) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (ctx->pending) return fail(ctx, RAYN_ERR_INVALID_ARG, "a render is already in flight on this context");
-  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "render_frame before upload_scene");
-  if (!f || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/out is NULL");
-  FramePlan P;
-  int32_t rc = frame_check(ctx, f, tiles_override != nullptr, &P);
+  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "%s before upload_scene", call);
+  return RAYN_OK;
+}
+
+// The job prologue: frame checks, tile list, stats reset, fence, input tables, scene plan, pass sizing and pass buffers.
+// render: a render, whose tiles are `tiles` or else the frame's own selection, and which restarts the debug queue log;
+// otherwise the albedo pass, which renders the whole tile grid.  out_space: where the job's output lives.
+static int32_t job_begin(RaynContext* ctx, const RaynFrameDesc* f, const std::vector<int>* tiles, bool render, int32_t out_space, Job* J) {
+  FramePlan& P = J->P;
+  int32_t rc = frame_check(ctx, f, tiles || !render, &P);
   if (rc) return rc;
-  DevFrame& fr = P.fr;
-  const int spp = fr.spp, mb = fr.max_bounces, np = P.np, wpc = P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit;
+  const DevFrame& fr = P.fr;
   const int stride = f->tile_stride > 0 ? f->tile_stride : 1;
   std::vector<int>& my_tiles = ctx->job_tiles;
   my_tiles.clear();
-  if (tiles_override) {
-    my_tiles = *tiles_override;
+  if (tiles) {
+    my_tiles = *tiles;
+  } else if (!render) {
+    for (int idx = 0; idx < fr.ntx * fr.nty; ++idx) my_tiles.push_back(idx);
   } else if (f->tile_list) {
     if (f->n_tile_list < 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "n_tile_list < 0");
     for (int i = 0; i < f->n_tile_list; ++i) {
@@ -757,46 +767,75 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   } else {
     for (int idx = f->tile_offset; idx < fr.ntx * fr.nty; idx += stride) my_tiles.push_back(idx);
   }
+  // the job's geometry, for render_finish once the caller has marked the job pending
+  ctx->job_w = f->width, ctx->job_h = f->height, ctx->job_tw = f->tile_w, ctx->job_th = f->tile_h, ctx->job_spp = fr.spp, ctx->job_nty = fr.nty;
 
   memset(&ctx->stats, 0, sizeof ctx->stats);
   ctx->timed_used = 0;
-  ctx->qlog.clear();
+  if (render) ctx->qlog.clear();
+  // Device-space pointers may have been produced on another stream (e.g. torch's): fence.
+  if (f->input_space == RAYN_MEM_DEVICE || out_space == RAYN_MEM_DEVICE) CU(cudaDeviceSynchronize());
+  CU(cudaEventRecord(ctx->ev0, ctx->stream));
+  if ((rc = upload_tables(ctx, f, &P.fr))) return rc;
+  if ((rc = scene_plan(ctx, &P))) return rc;
+  if ((rc = size_pass(ctx, P, my_tiles.size(), &J->tiles_per_pass))) return rc;
+  PassBufs& pb = J->pb = ctx->pb;
+  pb.R = P.R, pb.QS = P.QS, pb.tile_ids = ctx->d_tile_ids;
+  pb.lc_ns = P.lc_ns;
+  pb.seg_count = ctx->d_work_ctr + WC_SEG_COUNT;
+  CU(cudaMemsetAsync(pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), ctx->stream));
+  return RAYN_OK;
+}
+
+// Starts the pass over tiles [first, first + tiles_per_pass) of the job: uploads their ids.  The upload reads host memory,
+// so a render's graph capture begins after it.
+static int32_t pass_tiles(RaynContext* ctx, Job* J, size_t first) {
+  const int nt = J->pb.n_tiles = (int)std::min<size_t>(J->tiles_per_pass, ctx->job_tiles.size() - first);
+  CU(cudaMemcpyAsync(ctx->d_tile_ids, ctx->job_tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  return RAYN_OK;
+}
+
+// The pass's k_raygen, one thread per path.
+static void pass_raygen(RaynContext* ctx, const Job& J) {
+  ctx->stats.passes++;
+  timed_begin(ctx, RAYN_K_RAYGEN);
+  k_raygen<<<dim3((J.P.R + 255) / 256, J.pb.n_tiles), 256, 0, ctx->stream>>>(ctx->scene, J.P.fr, J.pb, J.P.n_fold);
+  timed_end(ctx, RAYN_K_RAYGEN);
+}
+
+// Enqueues one render on the context's stream.  Nothing here waits for the GPU (except the debug queue log), so a single
+// host thread can keep several GPUs busy (render_frame_multi).  tiles_override replaces the frame's own tile selection.
+// dev_planes_out (optional) receives the device-space planes the film was rendered into.
+static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
+                              RaynFilmPlanes* dev_planes_out) {
+  int32_t rc = job_ready(ctx, "render_frame");
+  if (rc) return rc;
+  if (!f || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/out is NULL");
+  Job J;
+  if ((rc = job_begin(ctx, f, tiles_override, true, out->space, &J))) return rc;
+  const FramePlan& P = J.P;
+  const DevFrame& fr = P.fr;
+  PassBufs& pb = J.pb;
+  const std::vector<int>& my_tiles = ctx->job_tiles;
+  const int mb = fr.max_bounces, np = P.np, wpc = P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
+  const int* sdf_idx = ctx->scene.sdf_idx;
+  const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, volume_on = P.volume_on;
   cudaStream_t st = ctx->stream;
 
-  // Device-space pointers may have been produced on another stream (e.g. torch's): fence.
-  if (f->input_space == RAYN_MEM_DEVICE || out->space == RAYN_MEM_DEVICE) CU(cudaDeviceSynchronize());
-  CU(cudaEventRecord(ctx->ev0, st));
-
-  if ((rc = upload_tables(ctx, f, &fr))) return rc;
   const size_t npx = (size_t)f->width * f->height;
-  float *p_color, *p_alpha, *p_bg, *p_normal;
+  RaynFilmPlanes dp = *out;  // the device-space planes the film is rendered into
   if (out->space == RAYN_MEM_HOST) {
     CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 10));
     CU(cudaMemsetAsync(ctx->d_planes, 0, npx * 10 * 4, st));
-    p_color = ctx->d_planes, p_alpha = p_color + 3 * npx, p_bg = p_alpha + npx, p_normal = p_bg + 3 * npx;
+    dp = film_block_planes(ctx->d_planes, npx);
   } else {
-    p_color = out->color, p_alpha = out->alpha, p_bg = out->background, p_normal = out->normal;
     const int cov_w = std::min(fr.ntx * f->tile_w, f->width), cov_h = std::min(fr.nty * f->tile_h, f->height);
     if (cov_w < f->width || cov_h < f->height)
-      k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, p_color, p_alpha, p_bg, p_normal);
+      k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, dp.color, dp.alpha, dp.background, dp.normal);
   }
-  if (dev_planes_out) {
-    dev_planes_out->color = p_color, dev_planes_out->alpha = p_alpha, dev_planes_out->background = p_bg, dev_planes_out->normal = p_normal;
-    dev_planes_out->space = RAYN_MEM_DEVICE;
-  }
+  dp.space = RAYN_MEM_DEVICE;
+  if (dev_planes_out) *dev_planes_out = dp;
 
-  if ((rc = scene_plan(ctx, &P))) return rc;
-  const int n_sdf = P.n_sdf, n_fold = P.n_fold, lc_ns = P.lc_ns;
-  const int* sdf_idx = P.sdf_idx;
-  const bool simple = P.simple, motion = P.motion, traps = P.traps, volume_on = P.volume_on;
-
-  int tiles_per_pass;
-  if ((rc = size_pass(ctx, P, my_tiles.size(), &tiles_per_pass))) return rc;
-  PassBufs pb = ctx->pb;
-  pb.R = R, pb.QS = QS, pb.tile_ids = ctx->d_tile_ids;
-  pb.lc_ns = lc_ns;
-  pb.seg_count = ctx->d_work_ctr + WC_SEG_COUNT;
-  CU(cudaMemsetAsync(pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), st));
   const size_t res_smem = resolve_smem_per_warp(np) * wpc;
   int slot_bits = 5, depth_bits = 1;  // significant bits of a shading slot (< QS) and of a depth (<= max_bounces): what k_resolve's radix sort walks
   while ((1 << slot_bits) < QS + 1) ++slot_bits;
@@ -806,7 +845,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   // Small single-pass frames are launch bound (config 1: ~20 launches of a few microseconds each): capture the whole kernel
   // sequence of the pass once and replay it as ONE graph launch while nothing that is baked into the launches changes
   // (scene, frame geometry, every pointer, the tile set).
-  const bool single_pass = my_tiles.size() <= (size_t)tiles_per_pass;
+  const bool single_pass = my_tiles.size() <= (size_t)J.tiles_per_pass;
   const bool use_graph = single_pass && !my_tiles.empty() && !(ctx->flags & (RAYN_FLAG_TIMING | RAYN_FLAG_NO_GRAPH)) && !ctx->qlog_enabled &&
                          (int64_t)my_tiles.size() * R <= ((int64_t)8 << 20);
   bool capturing = false, replayed = false;
@@ -817,7 +856,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     key = fnv1a(1469598103934665603ull, &ctx->scene, sizeof ctx->scene);
     key = fnv1a(key, &fr, sizeof fr);
     key = fnv1a(key, &kpb, sizeof kpb);
-    float* planes4[4] = {p_color, p_alpha, p_bg, p_normal};
+    float* planes4[4] = {dp.color, dp.alpha, dp.background, dp.normal};
     key = fnv1a(key, planes4, sizeof planes4);
     const int misc[6] = {np, wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0};
     key = fnv1a(key, misc, sizeof misc);
@@ -830,23 +869,15 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     }
   }
   std::vector<int> h_nslots, h_slots;
-  for (size_t first = 0; first < my_tiles.size() && !replayed; first += tiles_per_pass) {
-    const int nt = (int)std::min<size_t>(tiles_per_pass, my_tiles.size() - first);
-    pb.n_tiles = nt;
-    CU(cudaMemcpyAsync(ctx->d_tile_ids, my_tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, st));
+  for (size_t first = 0; first < my_tiles.size() && !replayed; first += J.tiles_per_pass) {
+    if ((rc = pass_tiles(ctx, &J, first))) return rc;
     if (use_graph) {
       CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
       capturing = true;
     }
-    ctx->stats.passes++;
-    const dim3 g_paths((R + 255) / 256, nt), g_shade((QS + 127) / 128, nt);
-    // resident grids (one wave) of the kernels that stride over a work list (k_scan_slots / k_scan_live), capped by the list's upper bound
-    const int64_t max_blocks = (int64_t)nt * ((QS + SLOT_BLOCK - 1) / SLOT_BLOCK);
-    auto resident = [&](int occ) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((int64_t)ctx->n_sm * occ, max_blocks)); };
+    pass_raygen(ctx, J);
+    const int nt = pb.n_tiles;
     const int nseg = (QS + SEG_SLOTS - 1) / SEG_SLOTS;  // segments per tile of the queue kernels
-    timed_begin(ctx, RAYN_K_RAYGEN);
-    k_raygen<<<g_paths, 256, 0, st>>>(ctx->scene, fr, pb, n_fold);
-    timed_end(ctx, RAYN_K_RAYGEN);
     for (int depth = 0; depth <= mb; ++depth) {
       const Thr thr = make_thr(ctx->scene.cam, depth);
       if (simple) {
@@ -856,7 +887,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
         timed_end(ctx, RAYN_K_EXTEND);
 #endif
       } else {
-        if ((rc = extend_enqueue(ctx, P, pb, thr, resident(ctx->occ_sph)))) return rc;
+        if ((rc = extend_enqueue(ctx, J, thr))) return rc;
       }
       timed_begin(ctx, RAYN_K_BIN);
       k_bin_count<<<dim3(nseg, nt), BIN_T, 0, st>>>(pb, n_hit, nseg);
@@ -885,16 +916,16 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           const int v = ctx->sdf_var[sdf_idx[j]];
           timed_begin(ctx, RAYN_K_NORMALS);
           if ((ctx->scene.trap_mask >> h.material) & 1u)  // the bin's material has an orbit-trap albedo: normals + trap
-            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
+            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx, J, ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
           else
-            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
+            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx, J, ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
           timed_end(ctx, RAYN_K_NORMALS);
         }
         timed_begin(ctx, RAYN_K_SHADE_PRE);
         if (traps)
-          k_shade_pre<true><<<resident(ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+          k_shade_pre<true><<<resident(ctx, J, ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
         else
-          k_shade_pre<false><<<resident(ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+          k_shade_pre<false><<<resident(ctx, J, ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
         timed_end(ctx, RAYN_K_SHADE_PRE);
         if (ctx->scene.n_lights > 0) {
           for (int j = 0; j < n_sdf; ++j) {
@@ -906,14 +937,14 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
         }
         timed_begin(ctx, RAYN_K_SHADE_POST);
         if (traps)
-          k_shade_post<true><<<resident(ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+          k_shade_post<true><<<resident(ctx, J, ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
         else
-          k_shade_post<false><<<resident(ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+          k_shade_post<false><<<resident(ctx, J, ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
         timed_end(ctx, RAYN_K_SHADE_POST);
       } else {
 #ifdef RAYN_LEGACY_KERNELS
         timed_begin(ctx, RAYN_K_SHADE_PRE);
-        k_shade<<<g_shade, 128, 0, st>>>(ctx->scene, fr, pb, depth, thr);
+        k_shade<<<dim3((QS + 127) / 128, nt), 128, 0, st>>>(ctx->scene, fr, pb, depth, thr);
         timed_end(ctx, RAYN_K_SHADE_PRE);
 #endif
       }
@@ -925,7 +956,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
       }
     }
     timed_begin(ctx, RAYN_K_RESOLVE);
-    k_resolve<<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, p_color, p_alpha, p_bg, p_normal, np, wpc, slot_bits, depth_bits);
+    k_resolve<<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc, slot_bits, depth_bits);
     timed_end(ctx, RAYN_K_RESOLVE);
     if (capturing) {
       cudaGraph_t graph = nullptr;
@@ -944,22 +975,29 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     }
     CU(cudaGetLastError());
   }
-  ctx->job_w = f->width, ctx->job_h = f->height, ctx->job_tw = f->tile_w, ctx->job_th = f->tile_h, ctx->job_spp = spp, ctx->job_nty = fr.nty;
   ctx->pending = true;
+  return RAYN_OK;
+}
+
+// Copies the non-NULL planes of `user` between user memory and a device block of 10 floats per pixel (film_block_planes),
+// on the context's stream: kind cudaMemcpyHostToDevice fills the block, cudaMemcpyDeviceToHost reads it.
+static int32_t copy_planes(RaynContext* ctx, const RaynFilmPlanes& user, float* block, size_t npx, cudaMemcpyKind kind) {
+  const RaynFilmPlanes dev = film_block_planes(block, npx);
+  float* const u[4] = {user.color, user.alpha, user.background, user.normal};
+  float* const d[4] = {dev.color, dev.alpha, dev.background, dev.normal};
+  const bool h2d = kind == cudaMemcpyHostToDevice;
+  for (int i = 0; i < 4; ++i) {
+    if (!u[i]) continue;
+    const size_t bytes = npx * (i == 1 ? 1 : 3) * sizeof(float);  // alpha has one channel
+    CU(cudaMemcpyAsync(h2d ? d[i] : u[i], h2d ? u[i] : d[i], bytes, kind, ctx->stream));
+  }
   return RAYN_OK;
 }
 
 // D2H of host-space planes (after an optional gather), then the end-of-frame bookkeeping
 static int32_t copy_out_enqueue(RaynContext* ctx, const RaynFilmPlanes* out) {
   if (out->space != RAYN_MEM_HOST) return RAYN_OK;
-  cudaStream_t st = ctx->stream;
-  const size_t npx = (size_t)ctx->job_w * ctx->job_h;
-  const float* d = ctx->d_planes;
-  if (out->color) CU(cudaMemcpyAsync(out->color, d, npx * 3 * 4, cudaMemcpyDeviceToHost, st));
-  if (out->alpha) CU(cudaMemcpyAsync(out->alpha, d + 3 * npx, npx * 4, cudaMemcpyDeviceToHost, st));
-  if (out->background) CU(cudaMemcpyAsync(out->background, d + 4 * npx, npx * 3 * 4, cudaMemcpyDeviceToHost, st));
-  if (out->normal) CU(cudaMemcpyAsync(out->normal, d + 7 * npx, npx * 3 * 4, cudaMemcpyDeviceToHost, st));
-  return RAYN_OK;
+  return copy_planes(ctx, *out, ctx->d_planes, (size_t)ctx->job_w * ctx->job_h, cudaMemcpyDeviceToHost);
 }
 
 static int32_t render_finish(RaynContext* ctx) {
@@ -1115,26 +1153,16 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* f, const R
 // The first-hit albedo plane (statement in include/rayn_b200.h): the render's raygen and depth-0 closest-hit stage, then
 // k_albedo_paths and k_albedo_resolve (rt_albedo.cuh), pass by pass over the whole tile grid.  Never captured into a graph.
 int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float* albedo, int32_t space) {
-  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
-  if (ctx->pending) return fail(ctx, RAYN_ERR_INVALID_ARG, "a render is already in flight on this context");
-  if (!ctx->has_scene) return fail(ctx, RAYN_ERR_NO_SCENE, "render_albedo before upload_scene");
+  int32_t rc = job_ready(ctx, "render_albedo");
+  if (rc) return rc;
   if (!f || !albedo) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/albedo is NULL");
   if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_albedo: bad memory space %d", space);
   if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_albedo: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
-  FramePlan P;
-  int32_t rc = frame_check(ctx, f, true, &P);
-  if (rc) return rc;
-  DevFrame& fr = P.fr;
-  std::vector<int>& tiles = ctx->job_tiles;
-  tiles.clear();
-  for (int idx = 0; idx < fr.ntx * fr.nty; ++idx) tiles.push_back(idx);
-
-  memset(&ctx->stats, 0, sizeof ctx->stats);
-  ctx->timed_used = 0;
+  Job J;  // the render's own pass sizing: alternating renders and albedo passes reuse the same pass buffers
+  if ((rc = job_begin(ctx, f, nullptr, false, space, &J))) return rc;
+  const DevFrame& fr = J.P.fr;
+  const PassBufs& pb = J.pb;
   cudaStream_t st = ctx->stream;
-  if (f->input_space == RAYN_MEM_DEVICE || space == RAYN_MEM_DEVICE) CU(cudaDeviceSynchronize());
-  CU(cudaEventRecord(ctx->ev0, st));
-  if ((rc = upload_tables(ctx, f, &fr))) return rc;
   const size_t npx = (size_t)f->width * f->height;
   float* dst = albedo;
   if (space == RAYN_MEM_HOST) {
@@ -1142,36 +1170,19 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float*
     dst = ctx->d_planes;
   }
   CU(cudaMemsetAsync(dst, 0, npx * 3 * sizeof(float), st));  // pixels outside the tile grid stay 0
-  if ((rc = scene_plan(ctx, &P))) return rc;
-  int tiles_per_pass;  // the render's own sizing: alternating renders and albedo passes reuse the same pass buffers
-  if ((rc = size_pass(ctx, P, tiles.size(), &tiles_per_pass))) return rc;
-  PassBufs pb = ctx->pb;
-  pb.R = P.R, pb.QS = P.QS, pb.tile_ids = ctx->d_tile_ids;
-  pb.lc_ns = P.lc_ns;
-  pb.seg_count = ctx->d_work_ctr + WC_SEG_COUNT;
-  CU(cudaMemsetAsync(pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), st));
   const Thr thr = make_thr(ctx->scene.cam, 0);
-  for (size_t first = 0; first < tiles.size(); first += tiles_per_pass) {
-    const int nt = (int)std::min<size_t>(tiles_per_pass, tiles.size() - first);
-    pb.n_tiles = nt;
-    CU(cudaMemcpyAsync(ctx->d_tile_ids, tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, st));
-    ctx->stats.passes++;
-    const dim3 g_paths((P.R + 255) / 256, nt);
-    const int64_t max_blocks = (int64_t)nt * ((P.QS + SLOT_BLOCK - 1) / SLOT_BLOCK);
-    const unsigned sph_grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((int64_t)ctx->n_sm * ctx->occ_sph, max_blocks));
-    timed_begin(ctx, RAYN_K_RAYGEN);
-    k_raygen<<<g_paths, 256, 0, st>>>(ctx->scene, fr, pb, P.n_fold);
-    timed_end(ctx, RAYN_K_RAYGEN);
-    if ((rc = extend_enqueue(ctx, P, pb, thr, sph_grid))) return rc;
+  for (size_t first = 0; first < ctx->job_tiles.size(); first += J.tiles_per_pass) {
+    if ((rc = pass_tiles(ctx, &J, first))) return rc;
+    pass_raygen(ctx, J);
+    if ((rc = extend_enqueue(ctx, J, thr))) return rc;
     timed_begin(ctx, RAYN_K_NORMALS);
-    k_albedo_paths<<<g_paths, 256, 0, st>>>(ctx->scene, fr, pb, pb.nrm);
+    k_albedo_paths<<<dim3((J.P.R + 255) / 256, pb.n_tiles), 256, 0, st>>>(ctx->scene, fr, pb, pb.nrm);
     timed_end(ctx, RAYN_K_NORMALS);
     timed_begin(ctx, RAYN_K_RESOLVE);
-    k_albedo_resolve<<<dim3((f->tile_w * f->tile_h + 255) / 256, nt), 256, 0, st>>>(fr, pb, pb.nrm, dst);
+    k_albedo_resolve<<<dim3((f->tile_w * f->tile_h + 255) / 256, pb.n_tiles), 256, 0, st>>>(fr, pb, pb.nrm, dst);
     timed_end(ctx, RAYN_K_RESOLVE);
     CU(cudaGetLastError());
   }
-  ctx->job_w = f->width, ctx->job_h = f->height, ctx->job_tw = f->tile_w, ctx->job_th = f->tile_h, ctx->job_spp = fr.spp, ctx->job_nty = fr.nty;
   ctx->pending = true;
   if (space == RAYN_MEM_HOST) {
     const cudaError_t e = cudaMemcpyAsync(albedo, dst, npx * 3 * sizeof(float), cudaMemcpyDeviceToHost, st);
@@ -1362,23 +1373,22 @@ int32_t rayn_b200_film_postprocess(RaynContext* ctx, int32_t mode, int32_t W, in
   CU(cudaSetDevice(ctx->device));
   const size_t npx = (size_t)W * H, nbytes = npx * post_bytes_per_pixel(mode);
   cudaStream_t st = ctx->stream;
-  const float *c = pl->color, *a = pl->alpha, *b = pl->background, *n = pl->normal;
+  RaynFilmPlanes src = *pl;
   CU(cudaDeviceSynchronize());
-  if (pl->space == RAYN_MEM_HOST) {
+  if (pl->space == RAYN_MEM_HOST) {  // copies the planes the mode reads
     CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 10));
-    float* d = ctx->d_planes;
-    if (need_color) CU(cudaMemcpyAsync(d, pl->color, npx * 12, cudaMemcpyHostToDevice, st));
-    if (need_alpha) CU(cudaMemcpyAsync(d + 3 * npx, pl->alpha, npx * 4, cudaMemcpyHostToDevice, st));
-    if (need_bg) CU(cudaMemcpyAsync(d + 4 * npx, pl->background, npx * 12, cudaMemcpyHostToDevice, st));
-    if (need_normal) CU(cudaMemcpyAsync(d + 7 * npx, pl->normal, npx * 12, cudaMemcpyHostToDevice, st));
-    c = d, a = d + 3 * npx, b = d + 4 * npx, n = d + 7 * npx;
+    const RaynFilmPlanes used{need_color ? pl->color : nullptr, need_alpha ? pl->alpha : nullptr, need_bg ? pl->background : nullptr,
+                              need_normal ? pl->normal : nullptr, RAYN_MEM_HOST};
+    int32_t rc = copy_planes(ctx, used, ctx->d_planes, npx, cudaMemcpyHostToDevice);
+    if (rc) return rc;
+    src = film_block_planes(ctx->d_planes, npx);
   }
   unsigned char* dout = out;
   if (out_space == RAYN_MEM_HOST) {
     CU(regrow(&ctx->d_post, &ctx->cap_post, nbytes));
     dout = ctx->d_post;
   }
-  k_postprocess<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(mode, W, H, c, a, b, n, dout);
+  k_postprocess<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(mode, W, H, src.color, src.alpha, src.background, src.normal, dout);
   CU(cudaGetLastError());
   if (out_space == RAYN_MEM_HOST) CU(cudaMemcpyAsync(out, dout, nbytes, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -1408,13 +1418,11 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
   float* stage = scratch + (albedo ? 16 : 12) * npx;
   const float *c_in = in->color, *b_in = in->background, *n_in = in->normal, *a_in = in->alpha;
   if (in->space == RAYN_MEM_HOST) {
-    float* s = stage;
+    int32_t rc = copy_planes(ctx, *in, stage, npx, cudaMemcpyHostToDevice);
+    if (rc) return rc;
+    const RaynFilmPlanes s = film_block_planes(stage, npx);
     stage += 10 * npx;
-    CU(cudaMemcpyAsync(s, in->normal, npx * 12, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(s + 3 * npx, in->alpha, npx * 4, cudaMemcpyHostToDevice, st));
-    if (in->color) CU(cudaMemcpyAsync(s + 4 * npx, in->color, npx * 12, cudaMemcpyHostToDevice, st));
-    if (in->background) CU(cudaMemcpyAsync(s + 7 * npx, in->background, npx * 12, cudaMemcpyHostToDevice, st));
-    n_in = s, a_in = s + 3 * npx, c_in = in->color ? s + 4 * npx : nullptr, b_in = in->background ? s + 7 * npx : nullptr;
+    n_in = s.normal, a_in = s.alpha, c_in = in->color ? s.color : nullptr, b_in = in->background ? s.background : nullptr;
   }
   k_denoise_guides<<<blocks1d, 256, 0, st>>>((long long)npx, n_in, a_in, guide);
   if (albedo) {
@@ -1618,8 +1626,7 @@ int32_t rayn_b200_accum_round(RaynContext* ctx, RaynAccum* a, const RaynFrameDes
     if (a->K[t] + n_int > (1ll << 24))
       return fail(ctx, RAYN_ERR_INVALID_ARG, "accum_round: tile %d would hold %lld samples per pixel, more than 2^24", t, a->K[t] + n_int);
   }
-  RaynFilmPlanes dev{a->planes, a->planes + 3 * (size_t)a->W * a->H, a->planes + 4 * (size_t)a->W * a->H, a->planes + 7 * (size_t)a->W * a->H,
-                     RAYN_MEM_DEVICE};
+  const RaynFilmPlanes dev = film_block_planes(a->planes, (size_t)a->W * a->H);
   int32_t rc = render_enqueue(ctx, f, &dev, &active, nullptr);
   if (rc) return rc;
   if ((rc = render_finish(ctx))) return rc;
@@ -1658,18 +1665,16 @@ int32_t rayn_b200_accum_resolve(RaynContext* ctx, const RaynAccum* a, const Rayn
   const size_t npx = (size_t)a->W * a->H;
   float *c = out->color, *al = out->alpha, *b = out->background, *n = out->normal;
   if (out->space == RAYN_MEM_HOST) {  // resolve into the round's planes (free between rounds), then copy out
-    float* p = a->planes;
-    c = c ? p : nullptr, al = al ? p + 3 * npx : nullptr, b = b ? p + 4 * npx : nullptr, n = n ? p + 7 * npx : nullptr;
+    const RaynFilmPlanes p = film_block_planes(a->planes, npx);
+    c = c ? p.color : nullptr, al = al ? p.alpha : nullptr, b = b ? p.background : nullptr, n = n ? p.normal : nullptr;
   } else {
     CU(cudaDeviceSynchronize());  // device planes may still be in use on another stream (e.g. torch's)
   }
   k_accum_resolve<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(a->W, a->H, a->tw, a->th, a->ntx, a->nty, a->state, a->dt.K, c, al, b, n);
   CU(cudaGetLastError());
   if (out->space == RAYN_MEM_HOST) {
-    if (c) CU(cudaMemcpyAsync(out->color, c, npx * 12, cudaMemcpyDeviceToHost, st));
-    if (al) CU(cudaMemcpyAsync(out->alpha, al, npx * 4, cudaMemcpyDeviceToHost, st));
-    if (b) CU(cudaMemcpyAsync(out->background, b, npx * 12, cudaMemcpyDeviceToHost, st));
-    if (n) CU(cudaMemcpyAsync(out->normal, n, npx * 12, cudaMemcpyDeviceToHost, st));
+    int32_t rc = copy_planes(ctx, *out, a->planes, npx, cudaMemcpyDeviceToHost);
+    if (rc) return rc;
   }
   CU(cudaStreamSynchronize(st));
   return RAYN_OK;

@@ -77,6 +77,12 @@ struct PassBufs {
                       // allocated when the scene has traps (DevScene::trap_mask != 0), NULL otherwise
 };
 
+// The four film planes of a block of 10 floats per pixel: colour, alpha, background and normal at 0, 3, 4 and 7 floats
+// per pixel.  The staging of host-space planes and the accumulator's round planes use this layout.
+__host__ __device__ inline RaynFilmPlanes film_block_planes(float* block, size_t npx) {
+  return RaynFilmPlanes{block, block + 3 * npx, block + 4 * npx, block + 7 * npx, RAYN_MEM_DEVICE};
+}
+
 enum { CNT_EXTEND_RAYS = 0, CNT_SHADE_LANES = 1, CNT_SHADOW_RAYS = 2, CNT_EVALS_EXTEND = 3, CNT_EVALS_SHADOW = 4,
        CNT_BULB_ITERS_EXTEND = 5, CNT_BULB_ITERS_SHADOW = 6, CNT_EVALS_NORMALS = 7, CNT_TRIPS_EXTEND = 8, CNT_TRIPS_SHADOW = 9, CNT_TOTAL = 10 };  // Mandelbulb iterations actually run (the count is data dependent)
 

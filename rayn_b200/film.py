@@ -25,6 +25,13 @@ def _fptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
 
+def host_planes(width, height):
+    """Zeroed host planes of a width x height film (dict of flat float32 arrays, keyed by CHANNELS) and the host-space
+    RaynFilmPlanes that points at them.  Keep the dict alive while the C side may write the planes."""
+    planes = {k: np.zeros((1 if k == "alpha" else 3) * width * height, np.float32) for k in CHANNELS}
+    return planes, L.RaynFilmPlanes(*(planes[k].ctypes.data for k in CHANNELS), L.MEM_HOST)
+
+
 class FrameInputs:
     """Host-owned sampler state of one frame: `Samples::new_rd` tables (film.rs:434,
     sampler.rs:18-37), per-pixel SmallRng scramble (film.rs:460-461) and the
@@ -191,10 +198,7 @@ class Renderer:
     def render_host(self, inputs, tile_size, integrator, time_range, tile_offset=0, tile_stride=1, tile_list=None):
         """Host buffers in, host planes out (H2D + D2H inside the call).  Returns dict of numpy planes."""
         w, h = inputs.width, inputs.height
-        planes = {"color": np.zeros(3 * w * h, np.float32), "alpha": np.zeros(w * h, np.float32),
-                  "background": np.zeros(3 * w * h, np.float32), "normal": np.zeros(3 * w * h, np.float32)}
-        p = L.RaynFilmPlanes(planes["color"].ctypes.data, planes["alpha"].ctypes.data, planes["background"].ctypes.data,
-                             planes["normal"].ctypes.data, L.MEM_HOST)
+        planes, p = host_planes(w, h)
         ptrs = tuple(a.ctypes.data for a in inputs.arrays())
         f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST, tile_offset,
                             tile_stride, (inputs.sets_1d, inputs.sets_2d), tile_list)
@@ -273,10 +277,7 @@ class Renderer:
         (host or device) written in place."""
         planes = None
         if out is None:
-            npx = acc.width * acc.height
-            planes = {k: np.zeros((1 if k == "alpha" else 3) * npx, np.float32) for k in CHANNELS}
-            out = L.RaynFilmPlanes(planes["color"].ctypes.data, planes["alpha"].ctypes.data, planes["background"].ctypes.data,
-                                   planes["normal"].ctypes.data, L.MEM_HOST)
+            planes, out = host_planes(acc.width, acc.height)
         L.check(self._lib.rayn_b200_accum_resolve(self._ctx, acc.handle, C.byref(out)), self._ctx)
         return planes
 

@@ -56,14 +56,11 @@ def _f(a):
 def render(world, camera, inputs, tile_size, integrator, time_range, n_threads=0, subsample_k=1, tile_list=None, traps=None):
     """CPU render of the same FrameInputs with the world's orbit-trap albedos (World.albedo_traps(), or `traps`: a list of
     RaynAlbedoTrap).  Returns (planes dict, info dict), like oracle.binding.render."""
-    from rayn_b200.film import make_frame_desc
+    from rayn_b200.film import host_planes, make_frame_desc
     desc, keep = world.flatten(camera)
     traps = world.albedo_traps() if traps is None else traps
     w, h = inputs.width, inputs.height
-    planes = {"color": np.zeros(3 * w * h, np.float32), "alpha": np.zeros(w * h, np.float32),
-              "background": np.zeros(3 * w * h, np.float32), "normal": np.zeros(3 * w * h, np.float32)}
-    p = L.RaynFilmPlanes(planes["color"].ctypes.data, planes["alpha"].ctypes.data, planes["background"].ctypes.data,
-                         planes["normal"].ctypes.data, L.MEM_HOST)
+    planes, p = host_planes(w, h)
     ptrs = tuple(a.ctypes.data for a in inputs.arrays())
     f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST, 0, 1,
                         (inputs.sets_1d, inputs.sets_2d), tile_list)
