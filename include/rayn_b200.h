@@ -317,6 +317,27 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* frame,
 
 int32_t rayn_b200_get_stats(const RaynContext* ctx, RaynStats* out);
 
+/* ---- luminance second moments: a variance AOV (rayn_b200_film_denoise_variance, or an external filter) ----------------
+ * rayn_b200_render_frame plus two planes [W*H] (row-major, y up) in memory space `space`, which must equal out->space.
+ * In float, no contraction, with every product rounded on its own:
+ *   lum(v) = (0.2126f*v0 + 0.7152f*v1) + 0.0722f*v2
+ *   color_lum2 = (((+0 + lum(x_0)*lum(x_0)) + lum(x_1)*lum(x_1)) + ...) / (float)spp
+ * for every pixel of the tile grid (film.rs:399-404), the sum over the pixel's Color samples x_k in the order the film adds its
+ * Color samples (the reference's wavefront order, the order of the colour sums); background_lum2 the same over its Background
+ * samples.  Pixels outside the tile grid are 0 (device planes are cleared there, like the film planes).  A path adds at most
+ * one Color or Background sample, so this is the mean over the spp paths of the squared path luminance (0 for a path that
+ * added none): a film channel that adds like the others, so films of different sample counts combine by weighted averaging;
+ * with the film's mean and spp it gives the variance.  The film planes equal render_frame's bit for bit.  Any plane pointer
+ * of `out` or `moments` may be NULL, but not all six.  The tile selection, graph capture and asynchrony rules are render_frame's.
+ * RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.                                                                           */
+typedef struct RaynMomentPlanes {
+  float* color_lum2;      /* [W*H] */
+  float* background_lum2; /* [W*H] */
+  int32_t space;          /* RaynMemSpace */
+} RaynMomentPlanes;
+int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* frame, const RaynFilmPlanes* out,
+                                       const RaynMomentPlanes* moments);
+
 /* ---- first-hit albedo plane: an AOV for denoisers (rayn_b200_film_denoise_albedo, or an external one beside the
  * normal plane) -----------------------------------------------------------------------------------------------------
  * albedo[3*W*H] (row-major, y up, like the film planes) in memory space `space` (RaynMemSpace).  In float, no contraction:
@@ -436,6 +457,29 @@ int32_t rayn_b200_film_denoise(RaynContext* ctx, const RaynDenoiseDesc* desc, in
  * component gets a NaN e (skipped) or e = +inf (weight +0).                                                         */
 int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_albedo, const float* albedo,
                                       int32_t width, int32_t height, const RaynFilmPlanes* in, const RaynFilmPlanes* out);
+/* The same filter guided by each pixel's variance (after Schied et al., SVGF, HPG 2017; PAPERS.md).  Each colour plane X
+ * (color, background) is filtered with its moment plane M (color_lum2, background_lum2 of rayn_b200_render_frame_moments for
+ * a film of `spp` samples per pixel), lum() as stated there.  Every pixel carries (c, v); in float, in this order:
+ *   level 0:  v_p = fmaxf(M_p - lum(c_p)*lum(c_p), 0.0f) / (float)spp        (the variance of the pixel mean)
+ *   level i, pixel p with finite colour:
+ *     g_p  = (sum k*v_q) / (sum k) over the 3x3 taps q = p + (dx, dy), dx, dy in -1..1 (unit spacing, every level),
+ *            dy outer, dx inner, ascending, k = K[dy+1]*K[dx+1], K = {0.25, 0.5, 0.25}, skipping taps outside the image
+ *            and taps with a non-finite colour component
+ *     il_p = 1.0f / (sigma_luminance * sqrtf(g_p) + 1e-10f)
+ *     per tap of the 5x5 filter: e = e_0 + fabsf(lum(c_q) - lum(c_p)) * il_p, where e_0 is the e of rayn_b200_film_denoise,
+ *            or of rayn_b200_film_denoise_albedo when albedo != NULL; w, the skips and the colour output are unchanged
+ *     v'_p = (sum (w*w)*v_q) / (sw*sw), sw = sum w, the sum in tap order over the taps that are not skipped and whose w*w
+ *            is not +0
+ *   a pixel whose colour is non-finite is copied, colour and variance.  The last level writes the colour only.
+ * e stays a sum of non-negative terms or NaN (il_p is in [0, 1e10]), so the centre tap has e = 0 and w = h*h as before.
+ * sigma_luminance must be > 0; at +inf the term is not added, v is not formed, and the call equals
+ * rayn_b200_film_denoise (albedo NULL) or rayn_b200_film_denoise_albedo bit for bit.  albedo may be NULL (no albedo term);
+ * otherwise sigma_albedo follows rayn_b200_film_denoise_albedo.  spp >= 1.  `moments` lives in in->space
+ * (moments->space == in->space); a present input colour plane without its moment plane is RAYN_ERR_INVALID_ARG, as are
+ * spp < 1 and a bad sigma.  The aliasing, space and asynchrony rules are rayn_b200_film_denoise's.                       */
+int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_luminance, int32_t spp,
+                                        const RaynMomentPlanes* moments, float sigma_albedo, const float* albedo, int32_t width,
+                                        int32_t height, const RaynFilmPlanes* in, const RaynFilmPlanes* out);
 
 /* ---- progressive / adaptive rendering: a device film accumulator refined in sample rounds -----------------------
  * Per-tile stopping rule after Dammertz, Hanika, Keller, Lensch (WSCG 2009; PAPERS.md): a tile's error compares the

@@ -103,6 +103,10 @@ class RaynFilmPlanes(C.Structure):
                 ("normal", C.c_void_p), ("space", i32)]
 
 
+class RaynMomentPlanes(C.Structure):
+    _fields_ = [("color_lum2", C.c_void_p), ("background_lum2", C.c_void_p), ("space", i32)]
+
+
 class RaynDenoiseDesc(C.Structure):
     _fields_ = [("iterations", i32), ("sigma_color", f32), ("sigma_normal", f32), ("sigma_alpha", f32)]
 
@@ -156,6 +160,9 @@ SYMBOLS = {
     "rayn_b200_film_denoise_albedo": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, C.c_void_p, i32, i32, C.POINTER(RaynFilmPlanes),
                                             C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_render_albedo": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), C.c_void_p, i32]),
+    "rayn_b200_render_frame_moments": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes)]),
+    "rayn_b200_film_denoise_variance": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), f32, C.c_void_p, i32,
+                                              i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_accum_create": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(C.c_void_p)]),
     "rayn_b200_accum_destroy": (None, [C.c_void_p]),
     "rayn_b200_accum_round": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynAdaptiveDesc), C.POINTER(i32)]),

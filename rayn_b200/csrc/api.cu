@@ -92,6 +92,8 @@ struct RaynContext {
   size_t cap_s1 = 0, cap_s2 = 0, cap_scr = 0;
   float* d_planes = nullptr;
   size_t cap_planes = 0;
+  float* d_moments = nullptr;  // host-space moment planes of rayn_b200_render_frame_moments: 2 floats per pixel
+  size_t cap_moments = 0;
   int* d_pack_ids = nullptr;
   size_t cap_pack_ids = 0;
   unsigned char* d_post = nullptr;
@@ -306,7 +308,7 @@ static std::vector<int> shard_of(int W, int H, int tw, int th, int rank, int wor
 }
 
 static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
-                              RaynFilmPlanes* dev_planes_out);
+                              RaynFilmPlanes* dev_planes_out, const RaynMomentPlanes* moments = nullptr);
 static int32_t render_finish(RaynContext* ctx);
 static int32_t gather_enqueue(RaynContext* ctx, int W, int H, int tw, int th, const RaynFilmPlanes* pl, bool in_group);
 
@@ -398,6 +400,7 @@ void rayn_b200_destroy(RaynContext* ctx) {
   cudaFree(ctx->d_pack_ids);
   cudaFree(ctx->d_post);
   cudaFree(ctx->d_s1), cudaFree(ctx->d_s2), cudaFree(ctx->d_scr), cudaFree(ctx->d_fis), cudaFree(ctx->d_planes);
+  cudaFree(ctx->d_moments);
   for (auto& t : ctx->timed) cudaEventDestroy(t.a), cudaEventDestroy(t.b);
   if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
   cudaEventDestroy(ctx->ev0), cudaEventDestroy(ctx->ev1);
@@ -805,9 +808,10 @@ static void pass_raygen(RaynContext* ctx, const Job& J) {
 
 // Enqueues one render on the context's stream.  Nothing here waits for the GPU (except the debug queue log), so a single
 // host thread can keep several GPUs busy (render_frame_multi).  tiles_override replaces the frame's own tile selection.
-// dev_planes_out (optional) receives the device-space planes the film was rendered into.
+// dev_planes_out (optional) receives the device-space planes the film was rendered into.  moments (optional,
+// rayn_b200_render_frame_moments): the lum^2 planes, in out->space, which the k_resolve<true> instance also writes.
 static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const std::vector<int>* tiles_override,
-                              RaynFilmPlanes* dev_planes_out) {
+                              RaynFilmPlanes* dev_planes_out, const RaynMomentPlanes* moments) {
   int32_t rc = job_ready(ctx, "render_frame");
   if (rc) return rc;
   if (!f || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/out is NULL");
@@ -817,7 +821,8 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   const DevFrame& fr = P.fr;
   PassBufs& pb = J.pb;
   const std::vector<int>& my_tiles = ctx->job_tiles;
-  const int mb = fr.max_bounces, np = P.np, wpc = P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
+  const bool mom = moments != nullptr;
+  const int mb = fr.max_bounces, np = P.np, wpc = mom ? resolve_warps_per_cta(np, true) : P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
   const int* sdf_idx = ctx->scene.sdf_idx;
   const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, volume_on = P.volume_on;
   cudaStream_t st = ctx->stream;
@@ -835,12 +840,28 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   }
   dp.space = RAYN_MEM_DEVICE;
   if (dev_planes_out) *dev_planes_out = dp;
+  float *dm_color = nullptr, *dm_bg = nullptr;  // the device-space moment planes
+  if (mom) {
+    if (wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
+    if (moments->space == RAYN_MEM_HOST) {
+      CU(regrow(&ctx->d_moments, &ctx->cap_moments, npx * 2));
+      CU(cudaMemsetAsync(ctx->d_moments, 0, npx * 2 * 4, st));
+      dm_color = moments->color_lum2 ? ctx->d_moments : nullptr;
+      dm_bg = moments->background_lum2 ? ctx->d_moments + npx : nullptr;
+    } else {
+      dm_color = moments->color_lum2, dm_bg = moments->background_lum2;
+      const int cov_w = std::min(fr.ntx * f->tile_w, f->width), cov_h = std::min(fr.nty * f->tile_h, f->height);
+      if (cov_w < f->width || cov_h < f->height)  // the one-channel slot of k_zero_uncovered, once per plane
+        for (float* m : {dm_color, dm_bg})
+          if (m) k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, nullptr, m, nullptr, nullptr);
+    }
+  }
 
-  const size_t res_smem = resolve_smem_per_warp(np) * wpc;
+  const size_t res_smem = resolve_smem_per_warp(np, mom) * wpc;
   int slot_bits = 5, depth_bits = 1;  // significant bits of a shading slot (< QS) and of a depth (<= max_bounces): what k_resolve's radix sort walks
   while ((1 << slot_bits) < QS + 1) ++slot_bits;
   while ((1 << depth_bits) < mb + 1) ++depth_bits;
-  CU(cudaFuncSetAttribute(k_resolve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)res_smem));
+  CU(cudaFuncSetAttribute(mom ? k_resolve<true> : k_resolve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)res_smem));
 
   // Small single-pass frames are launch bound (config 1: ~20 launches of a few microseconds each): capture the whole kernel
   // sequence of the pass once and replay it as ONE graph launch while nothing that is baked into the launches changes
@@ -856,9 +877,9 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     key = fnv1a(1469598103934665603ull, &ctx->scene, sizeof ctx->scene);
     key = fnv1a(key, &fr, sizeof fr);
     key = fnv1a(key, &kpb, sizeof kpb);
-    float* planes4[4] = {dp.color, dp.alpha, dp.background, dp.normal};
-    key = fnv1a(key, planes4, sizeof planes4);
-    const int misc[6] = {np, wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0};
+    float* planes6[6] = {dp.color, dp.alpha, dp.background, dp.normal, dm_color, dm_bg};
+    key = fnv1a(key, planes6, sizeof planes6);
+    const int misc[7] = {np, wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0, mom ? 1 : 0};  // mom: the k_resolve instance
     key = fnv1a(key, misc, sizeof misc);
     key = fnv1a(key, my_tiles.data(), my_tiles.size() * sizeof(int));
     if (ctx->graph_exec && ctx->graph_key == key) {
@@ -956,7 +977,12 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
       }
     }
     timed_begin(ctx, RAYN_K_RESOLVE);
-    k_resolve<<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc, slot_bits, depth_bits);
+    if (mom)
+      k_resolve<true><<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc,
+                                                                                                     slot_bits, depth_bits, dm_color, dm_bg);
+    else
+      k_resolve<false><<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc,
+                                                                                                      slot_bits, depth_bits);
     timed_end(ctx, RAYN_K_RESOLVE);
     if (capturing) {
       cudaGraph_t graph = nullptr;
@@ -998,6 +1024,16 @@ static int32_t copy_planes(RaynContext* ctx, const RaynFilmPlanes& user, float* 
 static int32_t copy_out_enqueue(RaynContext* ctx, const RaynFilmPlanes* out) {
   if (out->space != RAYN_MEM_HOST) return RAYN_OK;
   return copy_planes(ctx, *out, ctx->d_planes, (size_t)ctx->job_w * ctx->job_h, cudaMemcpyDeviceToHost);
+}
+
+// D2H of host-space moment planes from their staging (ctx->d_moments: color_lum2, then background_lum2)
+static int32_t copy_moments_out(RaynContext* ctx, const RaynMomentPlanes* m) {
+  if (m->space != RAYN_MEM_HOST) return RAYN_OK;
+  const size_t npx = (size_t)ctx->job_w * ctx->job_h;
+  float* const dst[2] = {m->color_lum2, m->background_lum2};
+  for (int i = 0; i < 2; ++i)
+    if (dst[i]) CU(cudaMemcpyAsync(dst[i], ctx->d_moments + i * npx, npx * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  return RAYN_OK;
 }
 
 static int32_t render_finish(RaynContext* ctx) {
@@ -1144,6 +1180,24 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* f, const R
   if (rc) return rc;
   if ((rc = render_enqueue(ctx, f, out, nullptr, nullptr))) return rc;
   if ((rc = copy_out_enqueue(ctx, out))) {
+    render_finish(ctx);
+    return rc;
+  }
+  return render_finish(ctx);
+}
+
+// render_frame plus the lum^2 moment planes (statement in include/rayn_b200.h): the same job, with the k_resolve<true> instance
+int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* f, const RaynFilmPlanes* out, const RaynMomentPlanes* moments) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!out || !moments) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_frame_moments: out/moments is NULL");
+  if (!out->color && !out->alpha && !out->background && !out->normal && !moments->color_lum2 && !moments->background_lum2)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "render_frame_moments: every film and moment plane is NULL");
+  if ((out->space != RAYN_MEM_HOST && out->space != RAYN_MEM_DEVICE) || moments->space != out->space)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "render_frame_moments: the moment planes must be in the film planes' memory space");
+  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
+  int32_t rc = render_enqueue(ctx, f, out, nullptr, nullptr, moments);
+  if (rc) return rc;
+  if ((rc = copy_out_enqueue(ctx, out)) || (rc = copy_moments_out(ctx, moments))) {
     render_finish(ctx);
     return rc;
   }
@@ -1407,8 +1461,11 @@ static bool denoise_factor(float sigma, float* f) {
 // device copies of host-space inputs (10) and one host-space output channel (3), as the caller sized it.
 // albedo != NULL (rayn_b200_film_denoise_albedo with a finite sigma): the albedo plane in in->space and its factor il; the
 // scratch then holds 4 more floats per pixel (its float4 guide) after the ping-pong planes, and 3 more for a host-space plane.
+// mom != NULL (rayn_b200_film_denoise_variance with a finite sigma_luminance sl): the moment planes in in->space, 2 more
+// floats per pixel of staging when that is host memory; the variance travels in the .w lane of the ping-pong planes.
 static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W, int H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
-                               float ic0, float in_, float ia, float* scratch, const float* albedo = nullptr, float il = 0.0f) {
+                               float ic0, float in_, float ia, float* scratch, const float* albedo, float il, const RaynMomentPlanes* mom, float sl,
+                               int spp) {
   cudaStream_t st = ctx->stream;
   const size_t npx = (size_t)W * H;
   const unsigned blocks1d = (unsigned)((npx + 255) / 256);
@@ -1434,26 +1491,36 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
     }
     k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, l_in, alb);
   }
+  const float *m_c = mom ? mom->color_lum2 : nullptr, *m_b = mom ? mom->background_lum2 : nullptr;
+  if (mom && in->space == RAYN_MEM_HOST) {
+    if (c_in) CU(cudaMemcpyAsync(stage, m_c, npx * 4, cudaMemcpyHostToDevice, st));
+    if (b_in) CU(cudaMemcpyAsync(stage + npx, m_b, npx * 4, cudaMemcpyHostToDevice, st));
+    m_c = stage, m_b = stage + npx;
+    stage += 2 * npx;
+  }
   CU(cudaGetLastError());
-  const dim3 blk(32, 8), grid((unsigned)((W + 31) / 32), (unsigned)((H + 7) / 8));
   for (int ch = 0; ch < 2; ++ch) {
     const float* src3 = ch == 0 ? c_in : b_in;
     if (!src3) continue;
     float* dst_user = ch == 0 ? out->color : out->background;
     float* dst3 = out->space == RAYN_MEM_HOST ? stage : dst_user;
-    k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ping[0]);
+    if (mom)
+      k_denoise_pack_var<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ch == 0 ? m_c : m_b, (float)spp, ping[0]);
+    else
+      k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ping[0]);
     for (int i = 0; i < d->iterations; ++i) {
       const float ic = ldexpf(ic0, i);
       const float4* src = ping[i & 1];
+      float4* dst4 = ping[(i + 1) & 1];
       const bool last = i == d->iterations - 1;
-      if (albedo && last)
-        k_denoise_level<true, true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, nullptr, dst3, alb, il);
+      if (albedo && mom)
+        denoise_level<true, true>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, sl);
       else if (albedo)
-        k_denoise_level<false, true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, ping[(i + 1) & 1], nullptr, alb, il);
-      else if (last)
-        k_denoise_level<true><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, nullptr, dst3);
+        denoise_level<true, false>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, 0.0f);
+      else if (mom)
+        denoise_level<false, true>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, sl);
       else
-        k_denoise_level<false><<<grid, blk, 0, st>>>(W, H, 1 << i, ic, in_, ia, guide, src, ping[(i + 1) & 1], nullptr);
+        denoise_level<false, false>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, 0.0f);
     }
     CU(cudaGetLastError());
     if (out->space == RAYN_MEM_HOST) CU(cudaMemcpyAsync(dst_user, dst3, npx * 12, cudaMemcpyDeviceToHost, st));
@@ -1461,9 +1528,10 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
   return RAYN_OK;
 }
 
-// rayn_b200_film_denoise and, with an albedo plane (albedo != NULL), rayn_b200_film_denoise_albedo
+// rayn_b200_film_denoise and, with an albedo plane (albedo != NULL), rayn_b200_film_denoise_albedo; with moment planes
+// (mom != NULL) and a finite sigma_luminance sl, rayn_b200_film_denoise_variance
 static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
-                            const float* albedo, float il) {
+                            const float* albedo, float il, const RaynMomentPlanes* mom = nullptr, float sl = 0.0f, int spp = 0) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!d || !in || !out || W <= 0 || H <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad argument");
   if (d->iterations < 1 || d->iterations > 8) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: iterations %d not in [1,8]", d->iterations);
@@ -1481,12 +1549,12 @@ static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t 
   if (!in->color && !in->background) return RAYN_OK;
   const size_t npx = (size_t)W * H;
   const size_t nfloat = npx * (12 + (in->space == RAYN_MEM_HOST ? 10 : 0) + (out->space == RAYN_MEM_HOST ? 3 : 0) +
-                               (albedo ? 4 + (in->space == RAYN_MEM_HOST ? 3 : 0) : 0));
+                               (albedo ? 4 + (in->space == RAYN_MEM_HOST ? 3 : 0) : 0) + (mom && in->space == RAYN_MEM_HOST ? 2 : 0));
   cudaStream_t st = ctx->stream;
   float* scratch = nullptr;
   // stream-ordered and released below: nothing persists between calls (render-pass sizing reads cudaMemGetInfo)
   CU(cudaMallocAsync((void**)&scratch, nfloat * sizeof(float), st));
-  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il);
+  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il, mom, sl, spp);
   const cudaError_t ef = cudaFreeAsync(scratch, st);
   if (rc) return rc;
   CU(ef);
@@ -1509,6 +1577,25 @@ int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* d
                 sigma_albedo);
   // +inf: the term is not added at all (adding dl2 * 0 would turn a non-finite albedo tap into a NaN tap)
   return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il);
+}
+
+int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
+                                        float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                                        const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!moments || !in) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: moments/in is NULL");
+  if ((in->color && !moments->color_lum2) || (in->background && !moments->background_lum2))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: every input colour plane needs its moment plane");
+  if (moments->space != in->space) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: the moment planes must be in in->space");
+  if (spp < 1) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: spp %d < 1", spp);
+  if (!(sigma_luminance > 0.0f)) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: sigma_luminance %g must be > 0 (+inf disables the term)", sigma_luminance);
+  float il = 0.0f;
+  if (albedo && !denoise_factor(sigma_albedo, &il))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: sigma_albedo %g must be > 0 (+inf disables the term) and give a finite 1/sigma^2",
+                sigma_albedo);
+  // +inf: the term is not added (inf * sqrt(0) would be NaN), and the call is film_denoise / film_denoise_albedo
+  const bool var = !isinf(sigma_luminance);
+  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, var ? moments : nullptr, sigma_luminance, spp);
 }
 
 int32_t rayn_b200_device_frame_inputs(RaynContext* ctx, int32_t W, int32_t H, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,

@@ -25,6 +25,10 @@ namespace rt {
 
 __device__ __forceinline__ bool dn_finite3(const float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z); }
 
+// Luminance of the variance guide (rayn_b200_film_denoise_variance); the library builds with --fmad=false, so every product
+// is rounded on its own as the header states.
+__host__ __device__ __forceinline__ float dn_lum(float r, float g, float b) { return (0.2126f * r + 0.7152f * g) + 0.0722f * b; }
+
 // planes -> float4 (r, g, b, 0) / (nx, ny, nz, a)
 __global__ void __launch_bounds__(256) k_denoise_pack(long long npx, const float* __restrict__ c3, float4* __restrict__ out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -38,13 +42,28 @@ __global__ void __launch_bounds__(256) k_denoise_guides(long long npx, const flo
   out[i] = make_float4(n3[3 * i], n3[3 * i + 1], n3[3 * i + 2], a[i]);
 }
 
+// colour plane + its lum^2 moment plane -> float4 (r, g, b, v) with the level-0 variance of the pixel mean
+// v = fmaxf(M - lum(c)^2, 0) / spp
+__global__ void __launch_bounds__(256) k_denoise_pack_var(long long npx, const float* __restrict__ c3, const float* __restrict__ m, float fspp,
+                                                          float4* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npx) return;
+  const float r = c3[3 * i], g = c3[3 * i + 1], b = c3[3 * i + 2];
+  const float l = dn_lum(r, g, b);
+  out[i] = make_float4(r, g, b, fmaxf(m[i] - l * l, 0.0f) / fspp);
+}
+
 // One level with step 2^level.  kOut3: the last level writes the interleaved rgb output plane instead of a float4 plane.
 // kAlb (rayn_b200_film_denoise_albedo): a fourth edge-stopping term dl2 * il from the albedo guide, packed (r, g, b, 0) by
 // k_denoise_pack; the kAlb = false instances never read `alb` or `il` and run the code of rayn_b200_film_denoise.
-template <bool kOut3, bool kAlb = false>
+// kVar (rayn_b200_film_denoise_variance): src.w holds the pixel's variance v; a fifth term |lum(c_q) - lum(c_p)| * il_p with
+// il_p = 1 / (sl * sqrt(g_p) + 1e-10), g_p the 3x3 prefilter of v, and the output's .w is the filtered variance
+// (sum (w*w) v_q) / (sw*sw).  The prefilter is fused here: its 9 taps are neighbours of p that the 5x5 loop's first level
+// reads too, so they are L1 hits, and no extra plane or launch is needed.  The kVar = false instances never read `sl`.
+template <bool kOut3, bool kAlb = false, bool kVar = false>
 __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, float ic, float in_, float ia, const float4* __restrict__ guide,
                                                        const float4* __restrict__ src, float4* __restrict__ dst4, float* __restrict__ dst3,
-                                                       const float4* __restrict__ alb = nullptr, float il = 0.0f) {
+                                                       const float4* __restrict__ alb = nullptr, float il = 0.0f, float sl = 0.0f) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= W || y >= H) return;
   const size_t p = (size_t)y * W + x;
@@ -54,7 +73,29 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
     const float h[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
     const float4 gp = guide[p];
     const float4 lp = kAlb ? alb[p] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    float sr = 0.0f, sg = 0.0f, sb = 0.0f, sw = 0.0f;
+    float sr = 0.0f, sg = 0.0f, sb = 0.0f, sw = 0.0f, sv = 0.0f;
+    float lum_p = 0.0f, ilp = 0.0f;
+    if (kVar) {
+      lum_p = dn_lum(cp.x, cp.y, cp.z);
+      const float k3[3] = {0.25f, 0.5f, 0.25f};
+      float gs = 0.0f, gw = 0.0f;
+#pragma unroll
+      for (int dy = -1; dy <= 1; ++dy) {
+        const int qy = y + dy;
+        if (qy < 0 || qy >= H) continue;
+#pragma unroll
+        for (int dx = -1; dx <= 1; ++dx) {
+          const int qx = x + dx;
+          if (qx < 0 || qx >= W) continue;
+          const float4 cq = src[(size_t)qy * W + qx];
+          if (!dn_finite3(cq)) continue;
+          const float kk = k3[dy + 1] * k3[dx + 1];
+          gs += kk * cq.w;
+          gw += kk;
+        }
+      }
+      ilp = 1.0f / (sl * sqrtf(gs / gw) + 1e-10f);  // gw >= 0.25 (the centre tap is finite); ilp in [0, 1e10]
+    }
 #pragma unroll
     for (int dy = -2; dy <= 2; ++dy) {
       const int qy = y + step * dy;
@@ -85,6 +126,12 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
           const float dl2 = (ar * ar + ag * ag) + ab * ab;
           e = e + dl2 * il;
         }
+        if (kVar) {
+          // |dl| >= 0 or NaN times ilp in [0, 1e10] (v >= 0, so g >= 0 or +inf, sqrt(+inf) * sl = +inf gives ilp = 0): the term
+          // is >= 0 or NaN, never -0 < 0 or a 0 * inf, so e stays a sum of non-negative terms or NaN and both shortcuts hold
+          // (the centre tap still has e = 0).  A luminance that overflows to +-inf makes the term NaN or +inf: skipped or dead.
+          e = e + fabsf(dn_lum(cq.x, cq.y, cq.z) - lum_p) * ilp;
+        }
         if (!(e <= DENOISE_E_DEAD)) continue;  // NaN (skipped by the statement) or a weight of exactly +0 (argument above)
         const float hk = h[dy + 2] * h[dx + 2];
         const float w = e == 0.0f ? hk : hk * dm::exp(-e);
@@ -92,9 +139,15 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
         sg += w * cq.y;
         sb += w * cq.z;
         sw += w;
+        if (kVar && !kOut3) {  // the last level writes the colour only
+          // the statement adds only taps whose w*w is not +0 (so an infinite v_q never meets a zero weight); the dead taps
+          // skipped above have w = +0 and so add nothing there either
+          const float ww = w * w;
+          if (ww != 0.0f) sv += ww * cq.w;
+        }
       }
     }
-    o = make_float4(sr / sw, sg / sw, sb / sw, 0.0f);
+    o = make_float4(sr / sw, sg / sw, sb / sw, kVar && !kOut3 ? sv / (sw * sw) : 0.0f);
   }
   if (kOut3) {
     dst3[3 * p] = o.x;
@@ -103,6 +156,17 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
   } else {
     dst4[p] = o;
   }
+}
+
+// One level of the filter: the k_denoise_level instance of (last level, albedo guide, variance guide)
+template <bool kAlb, bool kVar>
+inline void denoise_level(cudaStream_t st, bool last, int W, int H, int step, float ic, float in_, float ia, const float4* guide, const float4* src,
+                          float4* dst4, float* dst3, const float4* alb, float il, float sl) {
+  const dim3 blk(32, 8), grid((unsigned)((W + 31) / 32), (unsigned)((H + 7) / 8));
+  if (last)
+    k_denoise_level<true, kAlb, kVar><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, nullptr, dst3, alb, il, sl);
+  else
+    k_denoise_level<false, kAlb, kVar><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, dst4, nullptr, alb, il, sl);
 }
 
 }  // namespace rt

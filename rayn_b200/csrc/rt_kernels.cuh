@@ -1168,12 +1168,13 @@ __global__ void __launch_bounds__(CMP_T) k_compact_scatter(const PassBufs pb, co
 #define RES_BINS 512  // histogram bins of the radix sort (digits of up to 9 bits)
 #define RES_ROW 33                       // staging rows are 32 entries + 1 pad: the channel lanes read their rows bank-conflict free
 #define RES_STAGE_FLOATS (6 * RES_ROW + 2)  // staging buffer of the ordered sums: up to 6 channel rows
+#define RES_STAGE_FLOATS_MOM (8 * RES_ROW + 2)  // k_resolve<true>: 2 more rows, the lum^2 of Color and Background paths
 // per warp: key[np] (by sample index), two index arrays (ping-pong of the radix sort), the histogram bins, the staging rows
-__host__ __device__ inline size_t resolve_smem_per_warp(int np) {
-  return (size_t)np * (sizeof(uint32_t) + 2 * sizeof(uint16_t)) + RES_BINS * sizeof(int) + RES_STAGE_FLOATS * sizeof(float);
+__host__ __device__ inline size_t resolve_smem_per_warp(int np, bool mom = false) {
+  return (size_t)np * (sizeof(uint32_t) + 2 * sizeof(uint16_t)) + RES_BINS * sizeof(int) + (mom ? RES_STAGE_FLOATS_MOM : RES_STAGE_FLOATS) * sizeof(float);
 }
-static inline int resolve_warps_per_cta(int np) {
-  int w = (int)((size_t)200 * 1024 / resolve_smem_per_warp(np));
+static inline int resolve_warps_per_cta(int np, bool mom = false) {
+  int w = (int)((size_t)200 * 1024 / resolve_smem_per_warp(np, mom));
   return w < 1 ? 0 : (w > RES_MAX_WARPS ? RES_MAX_WARPS : w);
 }
 // One warp sorts the n sample indices in src[] by key[index] ascending: LSD radix sort over the low key_bits bits, stable, in
@@ -1280,7 +1281,8 @@ RT_D int resolve_keys(const float4* __restrict__ nrm0, const uint32_t* __restric
 // Strictly sequential float sums over the n entries of order[] (the reference's accumulation order), channel lanes
 // [0, n_rows): row r of the staging buffer holds, for 32 entries at a time, the value lane r has to add - component r % 3 of
 // src[order[i]] if the entry's class matches the row's (`want_lo` for rows 0-2, `want_hi` for rows 3-5; < 0: every entry), else
-// +0.0f (an exact no-op: the accumulator can never be -0).  The payload is gathered by the whole warp (32 loads in flight, the
+// +0.0f (an exact no-op: the accumulator can never be -0).  n_rows = 8 (rayn_b200_render_frame_moments): rows 6 and 7 hold
+// lum(v)^2 of the same entry, v = src[order[i]].xyz, for the `want_lo` and `want_hi` classes.  The payload is gathered by the whole warp (32 loads in flight, the
 // next chunk already requested), so the sum itself is one dependent FADD chain per channel fed from shared memory.
 RT_D float resolve_sum(const float4* __restrict__ src, const uint32_t* __restrict__ term, const uint16_t* order, int n, int lane, int n_rows,
                        int want_lo, int want_hi, float* stage) {
@@ -1308,6 +1310,12 @@ RT_D float resolve_sum(const float4* __restrict__ src, const uint32_t* __restric
       stage[4 * RES_ROW + lane] = hi ? cur.y : 0.0f;
       stage[5 * RES_ROW + lane] = hi ? cur.z : 0.0f;
     }
+    if (n_rows > 6) {  // in float without contraction (the library builds with --fmad=false), as the header states
+      const float l = (0.2126f * cur.x + 0.7152f * cur.y) + 0.0722f * cur.z;
+      const float l2 = l * l;
+      stage[6 * RES_ROW + lane] = lo ? l2 : 0.0f;
+      stage[7 * RES_ROW + lane] = hi ? l2 : 0.0f;
+    }
     __syncwarp();
     const int m = min(32, n - base);
     if (lane < n_rows) {
@@ -1321,15 +1329,19 @@ RT_D float resolve_sum(const float4* __restrict__ src, const uint32_t* __restric
   }
   return acc;
 }
+// kMom (rayn_b200_render_frame_moments): lanes 6 and 7 also sum lum^2 of the Color and Background paths in the same order
+// into lum2_color / lum2_bg; the kMom = false instance never reads them and runs the code of rayn_b200_render_frame.
+template <bool kMom>
 __global__ void __launch_bounds__(RES_MAX_WARPS * 32) k_resolve(const DevFrame fr, const PassBufs pb, float* __restrict__ color,
                                                                  float* __restrict__ alpha, float* __restrict__ background,
                                                                  float* __restrict__ normal, const int np, const int wpc, const int slot_bits,
-                                                                 const int depth_bits) {
+                                                                 const int depth_bits, float* __restrict__ lum2_color = nullptr,
+                                                                 float* __restrict__ lum2_bg = nullptr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  unsigned char* mine = smem_raw + (size_t)warp * resolve_smem_per_warp(np);
+  unsigned char* mine = smem_raw + (size_t)warp * resolve_smem_per_warp(np, kMom);
   float* stage = reinterpret_cast<float*>(mine);
-  int* hist = reinterpret_cast<int*>(stage + RES_STAGE_FLOATS);
+  int* hist = reinterpret_cast<int*>(stage + (kMom ? RES_STAGE_FLOATS_MOM : RES_STAGE_FLOATS));
   uint32_t* key = reinterpret_cast<uint32_t*>(hist + RES_BINS);
   uint16_t* idx0 = reinterpret_cast<uint16_t*>(key + np);
   uint16_t* idx1 = idx0 + np;
@@ -1361,9 +1373,13 @@ __global__ void __launch_bounds__(RES_MAX_WARPS * 32) k_resolve(const DevFrame f
     __syncwarp();
     const uint16_t* order = unordered ? warp_radix_sort(key, idx0, idx1, nB, slot_bits + depth_bits, lane, hist) : idx0;
     __syncwarp();
-    const float acc = resolve_sum(rad, term, order, nB, lane, 6, (int)TERM_COLOR, (int)TERM_BACKGROUND, stage);
+    const float acc = resolve_sum(rad, term, order, nB, lane, kMom ? 8 : 6, (int)TERM_COLOR, (int)TERM_BACKGROUND, stage);
     float* dst = lane < 3 ? color : background;
     if (lane < 6 && dst) dst[3 * pix + lane % 3] = acc / div;
+    if (kMom) {
+      float* m = lane == 6 ? lum2_color : lum2_bg;
+      if ((lane == 6 || lane == 7) && m) m[pix] = acc / div;
+    }
   }
 }
 

@@ -17,8 +17,9 @@ from . import _lib as L
 from .scene import BlackmanHarrisFilter, PathTracingIntegrator
 
 CHANNELS = ("color", "alpha", "background", "normal")  # ChannelKind, film.rs:103-120
-# a Film may also hold the first-hit albedo plane (Renderer.render_albedo), which the reference has no channel for
-FILM_CHANNELS = CHANNELS + ("albedo",)
+# a Film may also hold the first-hit albedo plane (Renderer.render_albedo) and the luminance second moments of its colour
+# and background planes (Renderer.render_host(moments=True)), which the reference has no channels for
+FILM_CHANNELS = CHANNELS + ("albedo", "moments")
 
 
 def _fptr(a):
@@ -88,6 +89,13 @@ DENOISE_DEFAULTS = dict(sigma_color=2.5, sigma_normal=0.4, sigma_alpha=0.5)
 # spp, the first camera samples of the film's own sequences): first-hit albedo converges much faster than colour.
 DENOISE_ALBEDO_SIGMA = 0.2
 ALBEDO_SAMPLES = 16
+
+# The variance-guided filter (rayn_b200_film_denoise_variance): sigma_luminance and the sigma_color it is paired with, picked
+# by `tools/bench_variance.py` (DESIGN.md §4f) on config 3 at 96x96, grey and with the README palette: the lowest mean col+bg
+# MSE over 4, 16 and 64 spp films (0.35 and 0.33 of the unguided defaults' MSE, with the albedo guide).  The luminance term
+# replaces the global colour term, so sigma_color is +inf.
+DENOISE_LUMINANCE_SIGMA = 4.0
+DENOISE_VARIANCE_SIGMA_COLOR = float("inf")
 
 
 def denoise_desc(iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
@@ -195,14 +203,22 @@ class Renderer:
         L.check(self._lib.rayn_b200_get_stats(self._ctx, C.byref(s)), self._ctx)
         return s
 
-    def render_host(self, inputs, tile_size, integrator, time_range, tile_offset=0, tile_stride=1, tile_list=None):
-        """Host buffers in, host planes out (H2D + D2H inside the call).  Returns dict of numpy planes."""
+    def render_host(self, inputs, tile_size, integrator, time_range, tile_offset=0, tile_stride=1, tile_list=None, moments=False):
+        """Host buffers in, host planes out (H2D + D2H inside the call).  Returns dict of numpy planes.  moments=True: the
+        same render with its luminance second moments (include/rayn_b200.h: rayn_b200_render_frame_moments), returned as
+        "moments", float32 [H, W, 2] (color_lum2, background_lum2)."""
         w, h = inputs.width, inputs.height
         planes, p = host_planes(w, h)
         ptrs = tuple(a.ctypes.data for a in inputs.arrays())
         f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST, tile_offset,
                             tile_stride, (inputs.sets_1d, inputs.sets_2d), tile_list)
-        self.render(f, p)
+        if not moments:
+            self.render(f, p)
+            return planes
+        m = np.zeros((2, h * w), np.float32)
+        mp = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
+        L.check(self._lib.rayn_b200_render_frame_moments(self._ctx, C.byref(f), C.byref(p), C.byref(mp)), self._ctx)
+        planes["moments"] = np.ascontiguousarray(m.reshape(2, h, w).transpose(1, 2, 0))
         return planes
 
     def render_albedo(self, inputs, tile_size, integrator, time_range):
@@ -226,12 +242,14 @@ class Renderer:
         return out
 
     def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, albedo=None,
-                sigma_albedo=None):
+                sigma_albedo=None, moments=None, spp=None, sigma_luminance=None):
         """Edge-avoiding a-trous filter of the color and background planes (include/rayn_b200.h: rayn_b200_film_denoise).
         numpy planes in ("normal" and "alpha" required, "color" / "background" optional); returns new arrays for the
         colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term.
         albedo (a [3*W*H] plane, e.g. render_albedo's): the albedo-guided filter (rayn_b200_film_denoise_albedo) with
-        sigma_albedo, default DENOISE_ALBEDO_SIGMA."""
+        sigma_albedo, default DENOISE_ALBEDO_SIGMA.  moments (float32 [H, W, 2], render_host(moments=True)'s) with the film's
+        spp: the variance-guided filter (rayn_b200_film_denoise_variance) with sigma_luminance, default
+        DENOISE_LUMINANCE_SIGMA, and sigma_color defaulting to DENOISE_VARIANCE_SIGMA_COLOR; combinable with albedo."""
         for k in ("normal", "alpha"):
             if planes.get(k) is None:
                 raise ValueError(f"denoise needs the {k} guide plane")
@@ -242,12 +260,24 @@ class Renderer:
             return d[k].ctypes.data if k in d else None
         pin = L.RaynFilmPlanes(ptr(flat, "color"), ptr(flat, "alpha"), ptr(flat, "background"), ptr(flat, "normal"), L.MEM_HOST)
         pout = L.RaynFilmPlanes(ptr(outs, "color"), None, ptr(outs, "background"), None, L.MEM_HOST)
+        if moments is not None and spp is None:
+            raise ValueError("the variance-guided denoise needs the film's spp")
+        if moments is not None and sigma_color is None:
+            sigma_color = DENOISE_VARIANCE_SIGMA_COLOR
         desc = denoise_desc(iterations, sigma_color, sigma_normal, sigma_alpha)
-        if albedo is None:
+        sa = float(DENOISE_ALBEDO_SIGMA if sigma_albedo is None else sigma_albedo)
+        if moments is not None:
+            m = np.ascontiguousarray(np.asarray(moments, np.float32).reshape(height, width, 2).transpose(2, 0, 1)).reshape(2, -1)
+            mp = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
+            sl = float(DENOISE_LUMINANCE_SIGMA if sigma_luminance is None else sigma_luminance)
+            alb = None if albedo is None else np.ascontiguousarray(albedo, np.float32).reshape(-1)
+            L.check(self._lib.rayn_b200_film_denoise_variance(self._ctx, C.byref(desc), sl, int(spp), C.byref(mp), sa,
+                                                              None if alb is None else alb.ctypes.data, width, height, C.byref(pin),
+                                                              C.byref(pout)), self._ctx)
+        elif albedo is None:
             L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
         else:
             alb = np.ascontiguousarray(albedo, np.float32).reshape(-1)
-            sa = float(DENOISE_ALBEDO_SIGMA if sigma_albedo is None else sigma_albedo)
             L.check(self._lib.rayn_b200_film_denoise_albedo(self._ctx, C.byref(desc), sa, alb.ctypes.data, width, height, C.byref(pin),
                                                             C.byref(pout)), self._ctx)
         return {k: v.reshape(np.shape(planes[k])) for k, v in outs.items()}
@@ -391,6 +421,7 @@ class Film:
         self._renderer = None
         self._device = device
         self.last_stats = None
+        self.spp = None  # samples per pixel of the last render_frame_into (the "moments" channel's count)
 
     def render_frame_into(self, world, camera, integrator, filt, tile_size, frame, time_range, samples):
         """Drop-in for film.rs:382-395.  time_range = (start, end)."""
@@ -399,10 +430,13 @@ class Film:
         w, h = self.res
         inputs = FrameInputs(w, h, samples, integrator, filt, frame)
         self._renderer.upload_scene(world, camera)
-        planes = self._renderer.render_host(inputs, tile_size, integrator, time_range)
+        planes = self._renderer.render_host(inputs, tile_size, integrator, time_range, moments="moments" in self.channel_kinds)
         self.last_stats = self._renderer.stats()
+        self.spp = inputs.spp
         for k in self.channel_kinds:
-            if k != "albedo":
+            if k == "moments":
+                self.channels[k] = planes[k]
+            elif k != "albedo":
                 self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
         self._render_albedo(integrator, filt, tile_size, frame, time_range, samples)
         self.progressive_epoch += 1  # film.rs:657
@@ -424,6 +458,8 @@ class Film:
         like render_frame_into and sets self.tile_errors / self.tile_samples (per tile index tile_x * n_tiles_y + tile_y).
         on_round(film), if given, sees the film resolved after every round: a progressive preview.  Returns the number of
         rounds rendered."""
+        if "moments" in self.channel_kinds:
+            raise ValueError("render_adaptive does not fold luminance moments: use render_frame_into for a Film with \"moments\"")
         import torch  # device buffers for the sample tables and the scramble plane
         if self._renderer is None:
             self._renderer = Renderer(self._device)
@@ -483,6 +519,8 @@ class Film:
         flat = {k: np.ascontiguousarray(v, np.float32).reshape(-1) for k, v in self.channels.items()}
         written = []
         for kind in write_channels:
+            if kind == "moments":
+                raise ValueError("the moments channel is not an image: read Film.channels[\"moments\"]")
             if kind == "color":
                 if transparent_background and "color" in flat and "alpha" in flat:
                     mode, pil = L.POST_COLOR_ALPHA, "RGBA"
@@ -506,17 +544,26 @@ class Film:
             written.append(path)
         return written
 
-    def denoise(self, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, sigma_albedo=None):
+    def denoise(self, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, sigma_albedo=None, sigma_luminance=None):
         """Filters the Film's color and background channels in place (Renderer.denoise), guided by its normal and alpha
-        channels, and by its albedo channel if it has one (sigma_albedo, default DENOISE_ALBEDO_SIGMA).  Call it after
-        render_frame_into and before save_to."""
+        channels, by its albedo channel if it has one (sigma_albedo, default DENOISE_ALBEDO_SIGMA), and by each pixel's
+        variance if it has the moments channel (sigma_luminance, default DENOISE_LUMINANCE_SIGMA).  Call it after
+        render_frame_into and before save_to.  The moments describe the unfiltered render, so the variance-guided filter
+        removes the "moments" channel from self.channels (a later call filters without it; render_frame_into fills it
+        again)."""
         for k in ("normal", "alpha"):
             if k not in self.channels:
                 raise ValueError(f"Film.denoise needs the {k} channel")
         if self._renderer is None:
             self._renderer = Renderer(self._device)
         w, h = self.res
-        if "albedo" in self.channels:
+        if "moments" in self.channels:
+            self.channels.update(self._renderer.denoise(w, h, {k: self.channels.get(k) for k in CHANNELS}, iterations, sigma_color,
+                                                        sigma_normal, sigma_alpha, albedo=self.channels.get("albedo"),
+                                                        sigma_albedo=sigma_albedo, moments=self.channels["moments"], spp=self.spp,
+                                                        sigma_luminance=sigma_luminance))
+            del self.channels["moments"]  # M - lum(c)^2 of filtered colour is not the variance of anything
+        elif "albedo" in self.channels:
             self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha,
                                                         albedo=self.channels["albedo"], sigma_albedo=sigma_albedo))
         else:

@@ -1,7 +1,9 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
 //   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] [--denoise L]
-//             [--denoise-albedo] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out file.ppm] [--dump planes.bin]
+//             [--denoise-albedo] [--denoise-variance] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out file.ppm] [--dump planes.bin]
 // --denoise-albedo (with --denoise) renders the first-hit albedo plane as rayn_b200.film.Film does and guides the filter with it.
+// --denoise-variance (with --denoise, not with --adaptive) renders the frame with its luminance moments and weights each
+// pixel's colour by its own variance, as rayn_b200.film.Film does with a "moments" channel; combinable with --denoise-albedo.
 // --orbit-trap colours the fractal of configs 2-5 by orbit trap: albedo (R0 G0 B0) at trap LO, (R1 G1 B1) at HI
 // (include/rayn_b200.h, RaynAlbedoTrap; tools/trap_range.py prints a range for config 3).
 // Renders one frame (frame 1, shutter 1/24 at 24 fps: main.rs:47-49,61-62), prints the reference's
@@ -23,6 +25,8 @@ static constexpr float kDenoiseSigmaColor = 2.5f, kDenoiseSigmaNormal = 0.4f, kD
 // --denoise-albedo: rayn_b200/film.py DENOISE_ALBEDO_SIGMA and ALBEDO_SAMPLES (picked in DESIGN.md §4e)
 static constexpr float kDenoiseAlbedoSigma = 0.2f;
 static constexpr int kAlbedoSamples = 16;
+// --denoise-variance: rayn_b200/film.py DENOISE_LUMINANCE_SIGMA and DENOISE_VARIANCE_SIGMA_COLOR (picked in DESIGN.md §4f)
+static constexpr float kDenoiseLuminanceSigma = 4.0f, kDenoiseVarianceSigmaColor = INFINITY;
 
 // --adaptive: the library's defaults (rayn_b200/film.py ADAPTIVE_THRESHOLD / ADAPTIVE_MAX_ROUNDS, picked in DESIGN.md §4c)
 static constexpr float kAdaptiveThreshold = 0.025f;
@@ -71,7 +75,7 @@ static CameraHandle setup_single_sphere(World& world, float rx, float ry) {  // 
 int main(int argc, char** argv) {
   int config = 3, W = 1280, H = 720, samples = 2, bounces = 3;  // setup.rs:16,22,30 defaults
   int denoise = 0;  // a-trous levels run after the render, before --out / --dump; 0 = off
-  bool denoise_albedo = false;
+  bool denoise_albedo = false, denoise_variance = false;
   bool adaptive = false;  // --adaptive: rounds of --samples each until every tile's error <= threshold (at most --rounds)
   float threshold = kAdaptiveThreshold;
   int max_rounds = kAdaptiveMaxRounds;
@@ -89,6 +93,7 @@ int main(int argc, char** argv) {
     else if (!strcmp(argv[i], "--dump-scene") && i + 1 < argc) dump_scene = argv[++i];
     else if (!strcmp(argv[i], "--denoise") && i + 1 < argc) denoise = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--denoise-albedo")) denoise_albedo = true;
+    else if (!strcmp(argv[i], "--denoise-variance")) denoise_variance = true;
     else if (!strcmp(argv[i], "--adaptive") && i + 1 < argc) adaptive = true, threshold = (float)atof(argv[++i]);
     else if (!strcmp(argv[i], "--rounds") && i + 1 < argc) max_rounds = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--orbit-trap") && i + 8 < argc) {
@@ -98,12 +103,14 @@ int main(int argc, char** argv) {
       orbit_trap = true;
     } else {
       fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] "
-                      "[--denoise L [--denoise-albedo]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out f.ppm] [--dump f.bin]\n");
+                      "[--denoise L [--denoise-albedo] [--denoise-variance]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out f.ppm] [--dump f.bin]\n");
       return 2;
     }
   }
   if (denoise < 0 || denoise > 8) { fprintf(stderr, "--denoise takes 1..8 levels (0 = off)\n"); return 2; }
   if (denoise_albedo && !denoise) { fprintf(stderr, "--denoise-albedo needs --denoise L\n"); return 2; }
+  if (denoise_variance && !denoise) { fprintf(stderr, "--denoise-variance needs --denoise L\n"); return 2; }
+  if (denoise_variance && adaptive) { fprintf(stderr, "--denoise-variance needs one render: the adaptive accumulator keeps no moments\n"); return 2; }
   if (max_rounds < 2) { fprintf(stderr, "--rounds takes at least 2 rounds\n"); return 2; }
   static const int cfg_res[6][2] = {{0, 0}, {256, 256}, {1024, 1024}, {1920, 1080}, {2048, 2048}, {7680, 4320}};
   static const int cfg_samples[6] = {0, 1, 32, 128, 64, 256}, cfg_bounces[6] = {0, 2, 4, 8, 4, 8};
@@ -145,15 +152,19 @@ int main(int argc, char** argv) {
       printf("%dx%d, %d rounds of %d spp, %d bounces: %.1f spp per tile on average, %lld of %zu tiles below E = %g\n", W, H, rounds, 4 * samples,
              bounces, (double)total / (double)std::max<size_t>(film.tile_samples.size(), 1), (long long)done, film.tile_samples.size(), threshold);
     } else {
-      film.render_frame_into(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end, samples);
+      film.render_frame_into(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end, samples, denoise_variance);
       const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
       printf("Done in %.3f seconds.\n", secs);  // main.rs:79-82
       printf("%dx%d, %d spp, %d bounces: %.2f Msamples/s (device %.1f ms, %lld kernel launches)\n", W, H, 4 * samples, bounces,
              (double)film.stats.paths / secs / 1e6, film.stats.total_ms, (long long)film.stats.launches);
     }
-    if (denoise_albedo) {
+    if (denoise_albedo)
       film.render_albedo(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end,
                          std::min(adaptive ? samples * max_rounds : samples, kAlbedoSamples));
+    if (denoise_variance) {
+      film.denoise_variance(denoise, kDenoiseVarianceSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha, kDenoiseLuminanceSigma, denoise_albedo,
+                            kDenoiseAlbedoSigma);
+    } else if (denoise_albedo) {
       film.denoise_albedo(denoise, kDenoiseSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha, kDenoiseAlbedoSigma);
     } else if (denoise) {
       film.denoise(denoise, kDenoiseSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha);

@@ -267,9 +267,10 @@ class Film {
   Film(const Film&) = delete;
   Film& operator=(const Film&) = delete;
 
-  // film.rs:382-395
+  // film.rs:382-395.  moments: the same render with its luminance second moments (rayn_b200_render_frame_moments) into
+  // color_lum2 / background_lum2, for denoise_variance; the film planes are the same.
   void render_frame_into(const World& world, CameraHandle camera, const PathTracingIntegrator& integrator, const BlackmanHarrisFilter& filter,
-                         int tile_w, int tile_h, int frame, float t0, float t1, int samples) {
+                         int tile_w, int tile_h, int frame, float t0, float t1, int samples, bool moments = false) {
     const int spp = 4 * samples;
     const int sets_1d = 1 + integrator.requested_1d_sample_sets();  // film.rs:431
     const int sets_2d = 2 + integrator.requested_2d_sample_sets();  // film.rs:432
@@ -281,7 +282,15 @@ class Film {
     RaynFrameDesc f = frame_desc(integrator, tile_w, tile_h, frame, t0, t1, samples, sets_1d, sets_2d);
     f.samples_1d = s1.data(), f.samples_2d = s2.data(), f.scramble = scr.data(), f.fis_inverse_cdf = fis.data();
     RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
-    check(rayn_b200_render_frame(ctx_, &f, &p), ctx_);
+    spp_ = spp;
+    if (moments) {
+      color_lum2.assign((size_t)w_ * h_, 0.0f), background_lum2.assign((size_t)w_ * h_, 0.0f);
+      const RaynMomentPlanes m{color_lum2.data(), background_lum2.data(), RAYN_MEM_HOST};
+      check(rayn_b200_render_frame_moments(ctx_, &f, &p, &m), ctx_);
+    } else {
+      color_lum2.clear(), background_lum2.clear();
+      check(rayn_b200_render_frame(ctx_, &f, &p), ctx_);
+    }
     rayn_b200_get_stats(ctx_, &stats);
     ++progressive_epoch;  // film.rs:657
   }
@@ -354,10 +363,25 @@ class Film {
     RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
     check(rayn_b200_film_denoise_albedo(ctx_, &d, sigma_albedo, albedo.data(), w_, h_, &p, &p), ctx_);
   }
+  // ... guided by each pixel's variance from the moments of render_frame_into(..., moments = true) and the film's spp
+  // (rayn_b200_film_denoise_variance), and by the albedo plane of render_albedo if with_albedo.  The moments describe the
+  // unfiltered film, so they are dropped once it is filtered (like rayn_b200.film.Film.denoise).
+  void denoise_variance(int iterations, float sigma_color, float sigma_normal, float sigma_alpha, float sigma_luminance, bool with_albedo,
+                        float sigma_albedo) {
+    if (color_lum2.empty()) throw std::runtime_error("denoise_variance needs a render_frame_into(..., moments = true) first");
+    if (with_albedo && albedo.empty()) throw std::runtime_error("denoise_variance with the albedo guide needs render_albedo first");
+    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    const RaynMomentPlanes m{color_lum2.data(), background_lum2.data(), RAYN_MEM_HOST};
+    check(rayn_b200_film_denoise_variance(ctx_, &d, sigma_luminance, spp_, &m, sigma_albedo, with_albedo ? albedo.data() : nullptr, w_, h_, &p, &p),
+          ctx_);
+    color_lum2.clear(), background_lum2.clear();
+  }
   int width() const { return w_; }
   int height() const { return h_; }
   std::vector<float> color, alpha, background, normal;
   std::vector<float> albedo;          // render_albedo: [3*W*H]
+  std::vector<float> color_lum2, background_lum2;  // render_frame_into(..., moments = true): [W*H] each
   std::vector<double> tile_errors;    // render_adaptive: E per tile index tile_x * n_tiles_y + tile_y
   std::vector<int64_t> tile_samples;  // ... and samples per pixel
   RaynStats stats{};
@@ -389,6 +413,7 @@ class Film {
     return f;
   }
   int w_, h_;
+  int spp_ = 0;  // samples per pixel of the last render_frame_into
   RaynContext* ctx_ = nullptr;
 };
 
