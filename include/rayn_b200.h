@@ -360,6 +360,35 @@ int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* fr
  * Lambertian / Dielectric hits, and a sum of nA ones is nA exactly.                                                 */
 int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, float* albedo /* [3*W*H] */, int32_t space);
 
+/* ---- screen-space motion of the first hit: the reprojection input of rayn_b200_temporal_push ----------------------------
+ * motion[4*W*H] (row-major, y up; per pixel dx, dy, z, z_prev) and optionally albedo[3*W*H], both in memory space `space`.
+ * Every camera sample s of a pixel of the tile grid is traced to render_frame's depth-0 hit exactly as in
+ * rayn_b200_render_albedo (same rays, same fold; frame->tile_list / tile_offset / tile_stride are ignored).  With tau the
+ * time of lane 0 of the sample's camera packet (the time raygen evaluates the camera at), in float, no contraction beyond the
+ * build's mul_add (fma3s / dot / cross / normalized of rt_device.cuh):
+ *   P  = fma3s(d, t, o)                                     the hit point, as rayn_b200_render_albedo forms it
+ *   P' = (P.x - v.x*frame_dt, P.y - v.y*frame_dt, P.z - v.z*frame_dt)   if the hit is a sphere with a non-zero
+ *        center_velocity v (each product rounded on its own); P' = P otherwise
+ *   proj(X, time) with the scene camera's origin, at, up evaluated at `time` as camera_ray does (a zero velocity keeps the
+ *        base value itself) and r = X - origin:
+ *     pinhole / thin lens (through the lens centre): bw = normalized(origin - at), bu = normalized(cross(up, bw)),
+ *        bv = cross(bw, bu), z = -dot(r, bw), px = ((dot(r, bu) / (z * hx)) * 0.5f + 0.5f) * (float)W,
+ *        py = ((dot(r, bv) / (z * hy)) * 0.5f + 0.5f) * (float)H
+ *     orthographic: bw = normalized(at - origin), bu = normalized(cross(bw, up)), bv = cross(bu, bw), z = dot(r, bw),
+ *        px = ((dot(r, bu) + hx) / full_size[0]) * (float)W, py = ((dot(r, bv) + hy) / full_size[1]) * (float)H
+ *     (hx, hy = half_size): the inverse of camera_ray's pixel -> (u, v) map, px = u * W, in film pixels
+ *   (px1, py1, z)      = proj(P, tau),  (px0, py0, z_prev) = proj(P', tau - frame_dt)
+ *   the sample is VALID if it hit something and, for a pinhole / thin-lens camera, z > 0 and z_prev > 0; its record is
+ *   (px0 - px1, py0 - py1, z, z_prev), and an invalid sample's record is (0, 0, NaN, NaN) (so a NaN z also counts invalid).
+ * motion[4p + k] = (((+0 + r_a[k]) + r_b[k]) + ...) / (float)n over the n valid samples of the pixel in ascending sample
+ * order; a pixel with n = 0, or outside the tile grid, is (0, 0, +inf, +inf), which never matches a history tap.
+ * Both projections are the same function, so a static camera and a static scene give dx = dy = +0 and z_prev == z exactly
+ * (tested).  If albedo != NULL it is rayn_b200_render_albedo's plane for the same frame, bit for bit, from the same march.
+ * frame_dt must be finite.  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; stats and graph rules are
+ * rayn_b200_render_albedo's (k_motion_paths counts under RAYN_K_NORMALS, k_motion_resolve under RAYN_K_RESOLVE).          */
+int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* frame, float frame_dt, float* motion /* [4*W*H] */,
+                                float* albedo /* [3*W*H] or NULL */, int32_t space);
+
 /* ---- multi-GPU: film tiles shard across GPUs, NCCL only for the final film gather -------------------------
  * The reference's only parallelism is one rayon task per tile over shared read-only state (film.rs:640-649); the
  * multi-GPU form of that is one context per GPU, each rendering the tiles `(tile_x + tile_y) % world == rank`
@@ -480,6 +509,55 @@ int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* d
 int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_luminance, int32_t spp,
                                         const RaynMomentPlanes* moments, float sigma_albedo, const float* albedo, int32_t width,
                                         int32_t height, const RaynFilmPlanes* in, const RaynFilmPlanes* out);
+/* rayn_b200_film_denoise_variance with a per-pixel variance scale (e.g. rayn_b200_temporal_push's var_scale, for a film that
+ * is a blend of frames): level 0 becomes
+ *   v_p = (fmaxf(M_p - lum(c_p)*lum(c_p), 0.0f) * scale_p) / (float)spp
+ * and everything else is unchanged.  var_scale [W*H] lives in in->space; NULL is RAYN_ERR_INVALID_ARG.  With var_scale == 1
+ * everywhere the call equals rayn_b200_film_denoise_variance bit for bit (x * 1 == x), and at sigma_luminance = +inf the
+ * scale is not read.                                                                                                       */
+int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_luminance, int32_t spp,
+                                               const RaynMomentPlanes* moments, const float* var_scale, float sigma_albedo,
+                                               const float* albedo, int32_t width, int32_t height, const RaynFilmPlanes* in,
+                                               const RaynFilmPlanes* out);
+
+/* ---- temporal accumulation of a frame sequence (the temporal half of SVGF, Schied et al. 2017; PAPERS.md) ---------------
+ * A RaynTemporal holds the reprojectable history of one W x H film: per pixel colour 3, background 3, the 2 moments,
+ * normal 3, z 1, history length n 1 and s 1, twice (14 floats per pixel each, allocated at create so render-pass sizing sees
+ * them; a push reads one and writes the other).  A new history has n = 0 everywhere.
+ * temporal_push(in, moments, motion): `in` is the current frame (color, background, normal required; alpha unused),
+ * `moments` its lum^2 planes (rayn_b200_render_frame_moments), `motion` its rayn_b200_render_motion plane.  Per pixel
+ * p = (x, y), in float, no contraction:
+ *   reset = 0 and z_prev finite:  fx = (((float)x + 0.5f) + dx) - 0.5f, fy likewise; x0 = floorf(fx), y0 = floorf(fy), ax = fx - x0, ay = fy - y0;
+ *     taps (x0 + i, y0 + j), j outer, i inner, in {0, 1}, weight w = (i ? ax : 1 - ax) * (j ? ay : 1 - ay).  A tap is USED if
+ *     w != 0, it is inside the image (compared in float), its history n > 0, its colour and background are finite,
+ *     fabsf(z_h - z_prev) <= sigma_depth * fabsf(z_prev) (so z_h is finite; |z_prev| serves orthographic views, whose z may
+ *     be <= 0) and ((nx_h*nx + ny_h*ny) + nz_h*nz) >= normal_cos (n the current normal).
+ *     ws = sum w, and every history value X (colour, background, moments, n, s) is X_h = (sum w*X_q) / ws, sums in tap order
+ *     over the used taps.  No used tap: n_h = 0.
+ *   reset = 1, or z_prev not finite (a pixel without a valid hit: motion (0, 0, +inf, +inf)):  n_h = 0.
+ *   alpha = fmaxf(alpha_min, 1.0f / (n_h + 1.0f));
+ *   alpha == 1 (always when n_h = 0): every output is the current frame's value bit for bit, n' = n_h + 1, s' = 1;
+ *   otherwise, for colour, background and both moments: x' = (1 - alpha) * x_h + alpha * x,  n' = n_h + 1,
+ *     s' = ((1 - alpha) * (1 - alpha)) * s_h + alpha * alpha.
+ * s' is the sum of squared blend weights: for frames with independent noise the variance of the blended pixel mean is
+ * max(M' - lum(c')^2, 0) * s' / spp, exact for this exponential moving average (a cumulative mean, alpha_min -> 0 on a static
+ * view, gives s' = 1/n').  The push writes c', b' to out, M' to out_moments and s' to var_scale, and stores c', b', M', n', s'
+ * with the current normal and z in the history.  out may alias in (each pixel reads only its own input).  Every plane and
+ * var_scale is required and in one memory space (in->space); host planes are staged and the call is synchronous, device
+ * planes run asynchronously on the context's stream (rayn_b200_sync waits).  RAYN_ERR_INVALID_ARG for a NULL plane, mixed
+ * spaces, or a bad desc.                                                                                                  */
+typedef struct RaynTemporal RaynTemporal;
+typedef struct RaynTemporalDesc {
+  float alpha_min;    /* (0, 1]: the smallest blend weight of the new frame                */
+  float sigma_depth;  /* > 0: relative depth tolerance of a history tap                     */
+  float normal_cos;   /* [-1, 1]: least dot product of history and current normal           */
+  int32_t reset;      /* 1: ignore the history (scene cut, first frame)                     */
+} RaynTemporalDesc;
+int32_t rayn_b200_temporal_create(RaynContext* ctx, int32_t width, int32_t height, RaynTemporal** out);
+void rayn_b200_temporal_destroy(RaynTemporal* t);
+int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* desc, const RaynFilmPlanes* in,
+                                const RaynMomentPlanes* moments, const float* motion, const RaynFilmPlanes* out,
+                                const RaynMomentPlanes* out_moments, float* var_scale);
 
 /* ---- progressive / adaptive rendering: a device film accumulator refined in sample rounds -----------------------
  * Per-tile stopping rule after Dammertz, Hanika, Keller, Lensch (WSCG 2009; PAPERS.md): a tile's error compares the

@@ -111,6 +111,10 @@ class RaynDenoiseDesc(C.Structure):
     _fields_ = [("iterations", i32), ("sigma_color", f32), ("sigma_normal", f32), ("sigma_alpha", f32)]
 
 
+class RaynTemporalDesc(C.Structure):
+    _fields_ = [("alpha_min", f32), ("sigma_depth", f32), ("normal_cos", f32), ("reset", i32)]
+
+
 class RaynAdaptiveDesc(C.Structure):
     _fields_ = [("min_rounds", i32), ("max_rounds", i32), ("threshold", f32)]
 
@@ -163,6 +167,13 @@ SYMBOLS = {
     "rayn_b200_render_frame_moments": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes)]),
     "rayn_b200_film_denoise_variance": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), f32, C.c_void_p, i32,
                                               i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_render_motion": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), f32, C.c_void_p, C.c_void_p, i32]),
+    "rayn_b200_film_denoise_variance_scaled": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), C.c_void_p, f32,
+                                                     C.c_void_p, i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_temporal_create": (i32, [C.c_void_p, i32, i32, C.POINTER(C.c_void_p)]),
+    "rayn_b200_temporal_destroy": (None, [C.c_void_p]),
+    "rayn_b200_temporal_push": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynTemporalDesc), C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes),
+                                      C.c_void_p, C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes), C.c_void_p]),
     "rayn_b200_accum_create": (i32, [C.c_void_p, i32, i32, i32, i32, C.POINTER(C.c_void_p)]),
     "rayn_b200_accum_destroy": (None, [C.c_void_p]),
     "rayn_b200_accum_round": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynFrameDesc), C.POINTER(RaynAdaptiveDesc), C.POINTER(i32)]),

@@ -17,6 +17,8 @@
 #include "rt_albedo.cuh"
 #include "rt_denoise.cuh"
 #include "rt_kernels.cuh"
+#include "rt_motion.cuh"
+#include "rt_temporal.cuh"
 #ifdef RAYN_LEGACY_KERNELS
 #include "rt_legacy.cuh"
 #endif
@@ -1248,6 +1250,59 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float*
   return render_finish(ctx);
 }
 
+// The first-hit motion plane and optionally the albedo plane (statement in include/rayn_b200.h): the albedo pass's job with
+// k_motion_paths and k_motion_resolve (rt_motion.cuh), and k_albedo_resolve on the same per-path albedos.  Never captured.
+int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, float* motion, float* albedo, int32_t space) {
+  int32_t rc = job_ready(ctx, "render_motion");
+  if (rc) return rc;
+  if (!f || !motion) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/motion is NULL");
+  if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_motion: bad memory space %d", space);
+  if (!isfinite(frame_dt)) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_motion: frame_dt %g is not finite", frame_dt);
+  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_motion: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
+  Job J;
+  if ((rc = job_begin(ctx, f, nullptr, false, space, &J))) return rc;
+  const DevFrame& fr = J.P.fr;
+  const PassBufs& pb = J.pb;
+  cudaStream_t st = ctx->stream;
+  const size_t npx = (size_t)f->width * f->height;
+  float *dm_ = motion, *da = albedo;
+  if (space == RAYN_MEM_HOST) {
+    CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 7));
+    dm_ = ctx->d_planes, da = albedo ? ctx->d_planes + 4 * npx : nullptr;
+  }
+  k_motion_clear<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>((long long)npx, dm_);  // pixels outside the tile grid
+  if (da) CU(cudaMemsetAsync(da, 0, npx * 3 * sizeof(float), st));
+  const Thr thr = make_thr(ctx->scene.cam, 0);
+  const dim3 paths_grid((J.P.R + 255) / 256, 1), pix_grid((f->tile_w * f->tile_h + 255) / 256, 1);
+  for (size_t first = 0; first < ctx->job_tiles.size(); first += J.tiles_per_pass) {
+    if ((rc = pass_tiles(ctx, &J, first))) return rc;
+    pass_raygen(ctx, J);
+    if ((rc = extend_enqueue(ctx, J, thr))) return rc;
+    const dim3 gp(paths_grid.x, pb.n_tiles), gr(pix_grid.x, pb.n_tiles);
+    timed_begin(ctx, RAYN_K_NORMALS);
+    if (da)
+      k_motion_paths<true><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
+    else
+      k_motion_paths<false><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
+    timed_end(ctx, RAYN_K_NORMALS);
+    timed_begin(ctx, RAYN_K_RESOLVE);
+    k_motion_resolve<<<gr, 256, 0, st>>>(fr, pb, pb.rad, dm_);
+    if (da) k_albedo_resolve<<<gr, 256, 0, st>>>(fr, pb, pb.nrm, da);
+    timed_end(ctx, RAYN_K_RESOLVE, da ? 2 : 1);
+    CU(cudaGetLastError());
+  }
+  ctx->pending = true;
+  if (space == RAYN_MEM_HOST) {
+    cudaError_t e = cudaMemcpyAsync(motion, dm_, npx * 4 * sizeof(float), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && albedo) e = cudaMemcpyAsync(albedo, da, npx * 3 * sizeof(float), cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) {
+      render_finish(ctx);
+      CU(e);
+    }
+  }
+  return render_finish(ctx);
+}
+
 int32_t rayn_b200_sync(RaynContext* ctx) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   CU(cudaSetDevice(ctx->device));
@@ -1463,9 +1518,11 @@ static bool denoise_factor(float sigma, float* f) {
 // scratch then holds 4 more floats per pixel (its float4 guide) after the ping-pong planes, and 3 more for a host-space plane.
 // mom != NULL (rayn_b200_film_denoise_variance with a finite sigma_luminance sl): the moment planes in in->space, 2 more
 // floats per pixel of staging when that is host memory; the variance travels in the .w lane of the ping-pong planes.
+// scale != NULL (rayn_b200_film_denoise_variance_scaled, with mom): the per-pixel variance scale in in->space, 1 more float per
+// pixel of staging when that is host memory.
 static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W, int H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
                                float ic0, float in_, float ia, float* scratch, const float* albedo, float il, const RaynMomentPlanes* mom, float sl,
-                               int spp) {
+                               int spp, const float* scale) {
   cudaStream_t st = ctx->stream;
   const size_t npx = (size_t)W * H;
   const unsigned blocks1d = (unsigned)((npx + 255) / 256);
@@ -1498,13 +1555,20 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
     m_c = stage, m_b = stage + npx;
     stage += 2 * npx;
   }
+  if (scale && in->space == RAYN_MEM_HOST) {
+    CU(cudaMemcpyAsync(stage, scale, npx * 4, cudaMemcpyHostToDevice, st));
+    scale = stage;
+    stage += npx;
+  }
   CU(cudaGetLastError());
   for (int ch = 0; ch < 2; ++ch) {
     const float* src3 = ch == 0 ? c_in : b_in;
     if (!src3) continue;
     float* dst_user = ch == 0 ? out->color : out->background;
     float* dst3 = out->space == RAYN_MEM_HOST ? stage : dst_user;
-    if (mom)
+    if (mom && scale)
+      k_denoise_pack_var<true><<<blocks1d, 256, 0, st>>>((long long)npx, src3, ch == 0 ? m_c : m_b, (float)spp, ping[0], scale);
+    else if (mom)
       k_denoise_pack_var<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ch == 0 ? m_c : m_b, (float)spp, ping[0]);
     else
       k_denoise_pack<<<blocks1d, 256, 0, st>>>((long long)npx, src3, ping[0]);
@@ -1529,9 +1593,11 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
 }
 
 // rayn_b200_film_denoise and, with an albedo plane (albedo != NULL), rayn_b200_film_denoise_albedo; with moment planes
-// (mom != NULL) and a finite sigma_luminance sl, rayn_b200_film_denoise_variance
+// (mom != NULL) and a finite sigma_luminance sl, rayn_b200_film_denoise_variance, and with a variance scale too (scale != NULL),
+// rayn_b200_film_denoise_variance_scaled
 static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
-                            const float* albedo, float il, const RaynMomentPlanes* mom = nullptr, float sl = 0.0f, int spp = 0) {
+                            const float* albedo, float il, const RaynMomentPlanes* mom = nullptr, float sl = 0.0f, int spp = 0,
+                            const float* scale = nullptr) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!d || !in || !out || W <= 0 || H <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad argument");
   if (d->iterations < 1 || d->iterations > 8) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: iterations %d not in [1,8]", d->iterations);
@@ -1549,12 +1615,13 @@ static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t 
   if (!in->color && !in->background) return RAYN_OK;
   const size_t npx = (size_t)W * H;
   const size_t nfloat = npx * (12 + (in->space == RAYN_MEM_HOST ? 10 : 0) + (out->space == RAYN_MEM_HOST ? 3 : 0) +
-                               (albedo ? 4 + (in->space == RAYN_MEM_HOST ? 3 : 0) : 0) + (mom && in->space == RAYN_MEM_HOST ? 2 : 0));
+                               (albedo ? 4 + (in->space == RAYN_MEM_HOST ? 3 : 0) : 0) + (mom && in->space == RAYN_MEM_HOST ? 2 : 0) +
+                               (mom && scale && in->space == RAYN_MEM_HOST ? 1 : 0));
   cudaStream_t st = ctx->stream;
   float* scratch = nullptr;
   // stream-ordered and released below: nothing persists between calls (render-pass sizing reads cudaMemGetInfo)
   CU(cudaMallocAsync((void**)&scratch, nfloat * sizeof(float), st));
-  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il, mom, sl, spp);
+  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il, mom, sl, spp, mom ? scale : nullptr);
   const cudaError_t ef = cudaFreeAsync(scratch, st);
   if (rc) return rc;
   CU(ef);
@@ -1579,9 +1646,10 @@ int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* d
   return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il);
 }
 
-int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
-                                        float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
-                                        const RaynFilmPlanes* out) {
+// rayn_b200_film_denoise_variance (scale NULL) and rayn_b200_film_denoise_variance_scaled
+static int32_t film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
+                                     const float* scale, float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                                     const RaynFilmPlanes* out) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!moments || !in) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: moments/in is NULL");
   if ((in->color && !moments->color_lum2) || (in->background && !moments->background_lum2))
@@ -1595,7 +1663,21 @@ int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc*
                 sigma_albedo);
   // +inf: the term is not added (inf * sqrt(0) would be NaN), and the call is film_denoise / film_denoise_albedo
   const bool var = !isinf(sigma_luminance);
-  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, var ? moments : nullptr, sigma_luminance, spp);
+  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, var ? moments : nullptr, sigma_luminance, spp, scale);
+}
+
+int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
+                                        float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                                        const RaynFilmPlanes* out) {
+  return film_denoise_variance(ctx, d, sigma_luminance, spp, moments, nullptr, sigma_albedo, albedo, W, H, in, out);
+}
+
+int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp,
+                                               const RaynMomentPlanes* moments, const float* var_scale, float sigma_albedo, const float* albedo,
+                                               int32_t W, int32_t H, const RaynFilmPlanes* in, const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!var_scale) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance_scaled: var_scale is NULL");
+  return film_denoise_variance(ctx, d, sigma_luminance, spp, moments, var_scale, sigma_albedo, albedo, W, H, in, out);
 }
 
 int32_t rayn_b200_device_frame_inputs(RaynContext* ctx, int32_t W, int32_t H, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,
@@ -1764,6 +1846,97 @@ int32_t rayn_b200_accum_resolve(RaynContext* ctx, const RaynAccum* a, const Rayn
     if (rc) return rc;
   }
   CU(cudaStreamSynchronize(st));
+  return RAYN_OK;
+}
+
+// ---- temporal accumulation (rt_temporal.cuh; statement in include/rayn_b200.h) -----------------------------------------
+struct RaynTemporal {
+  int device = 0, W = 0, H = 0;
+  float* hist[2] = {nullptr, nullptr};  // TH_PLANES planes of W*H floats each
+  int cur = 0;                          // the history the next push reads
+};
+
+int32_t rayn_b200_temporal_create(RaynContext* ctx, int32_t W, int32_t H, RaynTemporal** out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!out || W <= 0 || H <= 0 || (int64_t)W * H > ((int64_t)1 << 31)) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_create: bad argument");
+  *out = nullptr;
+  CU(cudaSetDevice(ctx->device));
+  RaynTemporal* t = new RaynTemporal();
+  t->device = ctx->device, t->W = W, t->H = H;
+  const size_t bytes = (size_t)W * H * TH_PLANES * sizeof(float);
+  cudaError_t e = cudaMalloc((void**)&t->hist[0], bytes);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&t->hist[1], bytes);
+  if (e == cudaSuccess) e = cudaMemsetAsync(t->hist[0], 0, bytes, ctx->stream);  // n = 0: no history yet
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(t->hist[0]), cudaFree(t->hist[1]);
+    delete t;
+    return fail(ctx, e == cudaErrorMemoryAllocation ? RAYN_ERR_OOM : RAYN_ERR_CUDA, "temporal_create (%dx%d): %s", W, H, cudaGetErrorString(e));
+  }
+  *out = t;
+  return RAYN_OK;
+}
+
+void rayn_b200_temporal_destroy(RaynTemporal* t) {
+  if (!t) return;
+  cudaSetDevice(t->device);
+  cudaDeviceSynchronize();
+  cudaFree(t->hist[0]), cudaFree(t->hist[1]);
+  delete t;
+}
+
+int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* d, const RaynFilmPlanes* in, const RaynMomentPlanes* mom,
+                                const float* motion, const RaynFilmPlanes* out, const RaynMomentPlanes* omom, float* scale) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!t || !d || !in || !mom || !motion || !out || !omom || !scale) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: NULL argument");
+  if (t->device != ctx->device) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: the history lives on device %d, the context on %d", t->device, ctx->device);
+  if (!in->color || !in->background || !in->normal || !mom->color_lum2 || !mom->background_lum2 || !out->color || !out->background ||
+      !omom->color_lum2 || !omom->background_lum2)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: the colour, background, normal and moment planes are required");
+  const int sp = in->space;
+  if ((sp != RAYN_MEM_HOST && sp != RAYN_MEM_DEVICE) || mom->space != sp || out->space != sp || omom->space != sp)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: every plane must be in one memory space");
+  if (!(d->alpha_min > 0.0f && d->alpha_min <= 1.0f) || !(d->sigma_depth > 0.0f) || !(d->normal_cos >= -1.0f && d->normal_cos <= 1.0f) ||
+      (d->reset != 0 && d->reset != 1))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: need alpha_min in (0, 1], sigma_depth > 0, normal_cos in [-1, 1], reset 0 or 1");
+  CU(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t npx = (size_t)t->W * t->H;
+  TemporalIo io{in->color, in->background, in->normal, mom->color_lum2, mom->background_lum2, motion,
+                out->color, out->background, omom->color_lum2, omom->background_lum2, scale};
+  float* stage = nullptr;
+  if (sp == RAYN_MEM_HOST) {  // stream-ordered staging, released within the call: 15 floats in, 9 out per pixel
+    CU(cudaMallocAsync((void**)&stage, npx * 24 * sizeof(float), st));
+    const float* src[6] = {in->color, in->background, in->normal, mom->color_lum2, mom->background_lum2, motion};
+    const int nf[6] = {3, 3, 3, 1, 1, 4};
+    const float** dst[6] = {&io.c, &io.b, &io.n, &io.mc, &io.mb, &io.motion};
+    float* s = stage;
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < 6; ++i) {
+      if (e == cudaSuccess) e = cudaMemcpyAsync(s, src[i], npx * nf[i] * sizeof(float), cudaMemcpyHostToDevice, st);
+      *dst[i] = s;
+      s += npx * nf[i];
+    }
+    io.oc = s, io.ob = s + 3 * npx, io.omc = s + 6 * npx, io.omb = s + 7 * npx, io.scale = s + 8 * npx;
+    if (e != cudaSuccess) {
+      cudaFreeAsync(stage, st);
+      CU(e);
+    }
+  }
+  k_temporal<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(t->W, t->H, *d, t->hist[t->cur], t->hist[t->cur ^ 1], io);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) t->cur ^= 1;
+  if (sp == RAYN_MEM_HOST) {
+    float* const udst[5] = {out->color, out->background, omom->color_lum2, omom->background_lum2, scale};
+    const float* const ddst[5] = {io.oc, io.ob, io.omc, io.omb, io.scale};
+    const int nf[5] = {3, 3, 1, 1, 1};
+    for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(udst[i], ddst[i], npx * nf[i] * sizeof(float), cudaMemcpyDeviceToHost, st);
+    const cudaError_t ef = cudaFreeAsync(stage, st);
+    if (e == cudaSuccess) e = ef;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  }
+  CU(e);
   return RAYN_OK;
 }
 

@@ -43,14 +43,17 @@ __global__ void __launch_bounds__(256) k_denoise_guides(long long npx, const flo
 }
 
 // colour plane + its lum^2 moment plane -> float4 (r, g, b, v) with the level-0 variance of the pixel mean
-// v = fmaxf(M - lum(c)^2, 0) / spp
+// v = fmaxf(M - lum(c)^2, 0) / spp; kScale (rayn_b200_film_denoise_variance_scaled): v = (fmaxf(M - lum(c)^2, 0) * scale) / spp
+template <bool kScale = false>
 __global__ void __launch_bounds__(256) k_denoise_pack_var(long long npx, const float* __restrict__ c3, const float* __restrict__ m, float fspp,
-                                                          float4* __restrict__ out) {
+                                                          float4* __restrict__ out, const float* __restrict__ scale = nullptr) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npx) return;
   const float r = c3[3 * i], g = c3[3 * i + 1], b = c3[3 * i + 2];
   const float l = dn_lum(r, g, b);
-  out[i] = make_float4(r, g, b, fmaxf(m[i] - l * l, 0.0f) / fspp);
+  float v = fmaxf(m[i] - l * l, 0.0f);
+  if (kScale) v = v * scale[i];
+  out[i] = make_float4(r, g, b, v / fspp);
 }
 
 // One level with step 2^level.  kOut3: the last level writes the interleaved rgb output plane instead of a float4 plane.

@@ -18,8 +18,9 @@ from .scene import BlackmanHarrisFilter, PathTracingIntegrator
 
 CHANNELS = ("color", "alpha", "background", "normal")  # ChannelKind, film.rs:103-120
 # a Film may also hold the first-hit albedo plane (Renderer.render_albedo) and the luminance second moments of its colour
-# and background planes (Renderer.render_host(moments=True)), which the reference has no channels for
-FILM_CHANNELS = CHANNELS + ("albedo", "moments")
+# and background planes (Renderer.render_host(moments=True)), which the reference has no channels for, and the first-hit
+# motion plane (Renderer.render_motion, float32 [H, W, 4]), which Film.render_sequence fills
+FILM_CHANNELS = CHANNELS + ("albedo", "moments", "motion")
 
 
 def _fptr(a):
@@ -96,6 +97,12 @@ ALBEDO_SAMPLES = 16
 # replaces the global colour term, so sigma_color is +inf.
 DENOISE_LUMINANCE_SIGMA = 4.0
 DENOISE_VARIANCE_SIGMA_COLOR = float("inf")
+# Temporal accumulation (Film.render_sequence, rayn_b200_temporal_push): picked by `tools/bench_temporal.py` (DESIGN.md §4g) by
+# the rule "lowest mean col+bg MSE over frames 9-24 of a 24-frame config-3 sequence with a moving camera, averaged over 4 and
+# 16 spp", over a grid of alpha_min, sigma_depth and normal_cos.
+# On one H100 80GB HBM3 (700 W, 1980 MHz): alpha_min 0.2, sigma_depth 0.1, normal_cos 0.5 gives 0.87x (4 spp) and 0.98x (16 spp) of
+# the spatial-only MSE, with 0.81x / 0.94x of its flicker.
+TEMPORAL_DEFAULTS = dict(alpha_min=0.2, sigma_depth=0.1, normal_cos=0.5)
 
 
 def denoise_desc(iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None):
@@ -142,6 +149,31 @@ class Accum:
     def close(self):
         if self._h:
             self._lib.rayn_b200_accum_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Temporal:
+    """The reprojectable history of one film (include/rayn_b200.h: rayn_b200_temporal_*), made by Renderer.temporal_create."""
+
+    def __init__(self, renderer, width, height):
+        self._lib = renderer._lib
+        self.width, self.height = width, height
+        self._h = C.c_void_p()
+        L.check(self._lib.rayn_b200_temporal_create(renderer.ctx, width, height, C.byref(self._h)), renderer.ctx)
+
+    @property
+    def handle(self):
+        return self._h
+
+    def close(self):
+        if self._h:
+            self._lib.rayn_b200_temporal_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -232,6 +264,42 @@ class Renderer:
         L.check(self._lib.rayn_b200_render_albedo(self._ctx, C.byref(f), out.ctypes.data, L.MEM_HOST), self._ctx)
         return out.reshape(h, w, 3)
 
+    def render_motion(self, inputs, tile_size, integrator, time_range, frame_dt, albedo=False):
+        """First-hit motion plane of the uploaded scene (include/rayn_b200.h: rayn_b200_render_motion) for host FrameInputs:
+        float32 [H, W, 4] (dx, dy, z, z_prev); albedo=True: (motion, render_albedo's [H, W, 3] plane from the same pass)."""
+        w, h = inputs.width, inputs.height
+        out = np.zeros(4 * w * h, np.float32)
+        alb = np.zeros(3 * w * h, np.float32) if albedo else None
+        ptrs = tuple(a.ctypes.data for a in inputs.arrays())
+        f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST,
+                            sets=(inputs.sets_1d, inputs.sets_2d))
+        L.check(self._lib.rayn_b200_render_motion(self._ctx, C.byref(f), float(frame_dt), out.ctypes.data,
+                                                  None if alb is None else alb.ctypes.data, L.MEM_HOST), self._ctx)
+        return (out.reshape(h, w, 4), alb.reshape(h, w, 3)) if albedo else out.reshape(h, w, 4)
+
+    def temporal_create(self, width, height):
+        return Temporal(self, width, height)
+
+    def temporal_push(self, t, planes, moments, motion, alpha_min, sigma_depth, normal_cos, reset=False):
+        """Blends one frame into the history t (include/rayn_b200.h: rayn_b200_temporal_push).  planes: numpy "color",
+        "background" and "normal"; moments float32 [H, W, 2]; motion float32 [H, W, 4] (render_motion's).  Returns
+        (planes with new "color" / "background", moments [H, W, 2], var_scale [H, W]) as float32 arrays."""
+        w, h = t.width, t.height
+        flat = {k: np.ascontiguousarray(planes[k], np.float32).reshape(-1) for k in ("color", "background", "normal")}
+        m = np.ascontiguousarray(np.asarray(moments, np.float32).reshape(h, w, 2).transpose(2, 0, 1)).reshape(2, -1)
+        mv = np.ascontiguousarray(motion, np.float32).reshape(-1)
+        oc, ob = np.empty_like(flat["color"]), np.empty_like(flat["background"])
+        om, scale = np.empty_like(m), np.empty(w * h, np.float32)
+        pin = L.RaynFilmPlanes(flat["color"].ctypes.data, None, flat["background"].ctypes.data, flat["normal"].ctypes.data, L.MEM_HOST)
+        pout = L.RaynFilmPlanes(oc.ctypes.data, None, ob.ctypes.data, None, L.MEM_HOST)
+        mi = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
+        mo = L.RaynMomentPlanes(om[0].ctypes.data, om[1].ctypes.data, L.MEM_HOST)
+        d = L.RaynTemporalDesc(float(alpha_min), float(sigma_depth), float(normal_cos), 1 if reset else 0)
+        L.check(self._lib.rayn_b200_temporal_push(self._ctx, t.handle, C.byref(d), C.byref(pin), C.byref(mi), mv.ctypes.data, C.byref(pout),
+                                                  C.byref(mo), scale.ctypes.data), self._ctx)
+        out = {"color": oc.reshape(np.shape(planes["color"])), "background": ob.reshape(np.shape(planes["background"]))}
+        return out, np.ascontiguousarray(om.reshape(2, h, w).transpose(1, 2, 0)), scale.reshape(h, w)
+
     def postprocess(self, mode, width, height, planes):
         """Film::save_to pixel arithmetic on the device (film.rs:205-377): numpy planes in, uint8 [H, W, bpp] out (rows top to bottom)."""
         def ptr(k):
@@ -242,14 +310,15 @@ class Renderer:
         return out
 
     def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, albedo=None,
-                sigma_albedo=None, moments=None, spp=None, sigma_luminance=None):
+                sigma_albedo=None, moments=None, spp=None, sigma_luminance=None, var_scale=None):
         """Edge-avoiding a-trous filter of the color and background planes (include/rayn_b200.h: rayn_b200_film_denoise).
         numpy planes in ("normal" and "alpha" required, "color" / "background" optional); returns new arrays for the
         colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term.
         albedo (a [3*W*H] plane, e.g. render_albedo's): the albedo-guided filter (rayn_b200_film_denoise_albedo) with
         sigma_albedo, default DENOISE_ALBEDO_SIGMA.  moments (float32 [H, W, 2], render_host(moments=True)'s) with the film's
         spp: the variance-guided filter (rayn_b200_film_denoise_variance) with sigma_luminance, default
-        DENOISE_LUMINANCE_SIGMA, and sigma_color defaulting to DENOISE_VARIANCE_SIGMA_COLOR; combinable with albedo."""
+        DENOISE_LUMINANCE_SIGMA, and sigma_color defaulting to DENOISE_VARIANCE_SIGMA_COLOR; combinable with albedo.
+        var_scale (float32 [H, W], temporal_push's), with moments: rayn_b200_film_denoise_variance_scaled."""
         for k in ("normal", "alpha"):
             if planes.get(k) is None:
                 raise ValueError(f"denoise needs the {k} guide plane")
@@ -271,9 +340,16 @@ class Renderer:
             mp = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
             sl = float(DENOISE_LUMINANCE_SIGMA if sigma_luminance is None else sigma_luminance)
             alb = None if albedo is None else np.ascontiguousarray(albedo, np.float32).reshape(-1)
-            L.check(self._lib.rayn_b200_film_denoise_variance(self._ctx, C.byref(desc), sl, int(spp), C.byref(mp), sa,
-                                                              None if alb is None else alb.ctypes.data, width, height, C.byref(pin),
-                                                              C.byref(pout)), self._ctx)
+            alb_p = None if alb is None else alb.ctypes.data
+            if var_scale is None:
+                L.check(self._lib.rayn_b200_film_denoise_variance(self._ctx, C.byref(desc), sl, int(spp), C.byref(mp), sa, alb_p, width, height,
+                                                                  C.byref(pin), C.byref(pout)), self._ctx)
+            else:
+                vs = np.ascontiguousarray(var_scale, np.float32).reshape(-1)
+                L.check(self._lib.rayn_b200_film_denoise_variance_scaled(self._ctx, C.byref(desc), sl, int(spp), C.byref(mp), vs.ctypes.data, sa,
+                                                                         alb_p, width, height, C.byref(pin), C.byref(pout)), self._ctx)
+        elif var_scale is not None:
+            raise ValueError("var_scale scales the variance of the moments: pass moments too")
         elif albedo is None:
             L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
         else:
@@ -436,7 +512,7 @@ class Film:
         for k in self.channel_kinds:
             if k == "moments":
                 self.channels[k] = planes[k]
-            elif k != "albedo":
+            elif k not in ("albedo", "motion"):  # "motion" is filled by render_sequence
                 self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
         self._render_albedo(integrator, filt, tile_size, frame, time_range, samples)
         self.progressive_epoch += 1  # film.rs:657
@@ -460,6 +536,8 @@ class Film:
         rounds rendered."""
         if "moments" in self.channel_kinds:
             raise ValueError("render_adaptive does not fold luminance moments: use render_frame_into for a Film with \"moments\"")
+        if "motion" in self.channel_kinds:
+            raise ValueError("render_adaptive renders no motion plane: use render_sequence for a Film with \"motion\"")
         import torch  # device buffers for the sample tables and the scramble plane
         if self._renderer is None:
             self._renderer = Renderer(self._device)
@@ -509,6 +587,62 @@ class Film:
         self.tile_errors, self.tile_samples = r.accum_tiles(acc)
         self.progressive_epoch += 1  # film.rs:657
 
+    def render_sequence(self, world, camera, integrator, filt, tile_size, frames, frame_rate, shutter, samples, iterations=5, on_frame=None,
+                        alpha_min=None, sigma_depth=None, normal_cos=None):
+        """Renders and denoises a frame sequence with temporal accumulation, like main.rs:58-97's frame loop: frame k covers
+        (k / frame_rate, k / frame_rate + shutter).  Per frame: a render with luminance moments; one motion pass (frame_dt =
+        1 / frame_rate) whose depth-0 march also gives the albedo plane if the Film has "albedo" (the first
+        4 * min(samples, ALBEDO_SAMPLES) samples, as render_frame_into's); the push into a film history (reset on the first
+        frame); the variance-guided denoise of the blend with its per-pixel variance scale; then on_frame(film).  The
+        temporal parameters default to TEMPORAL_DEFAULTS.  self.channels holds the denoised colour and background and the
+        frame's alpha, normal, albedo and motion planes (the ones the Film has).  Returns the number of frames."""
+        if "moments" in self.channel_kinds:
+            raise ValueError("render_sequence consumes the moments of every frame: create the Film without \"moments\"")
+        for k in ("color", "background", "alpha", "normal"):
+            if k not in self.channel_kinds:
+                raise ValueError(f"render_sequence needs the {k} channel")
+        t_kw = {k: float(TEMPORAL_DEFAULTS[k] if v is None else v)
+                for k, v in dict(alpha_min=alpha_min, sigma_depth=sigma_depth, normal_cos=normal_cos).items()}
+        if self._renderer is None:
+            self._renderer = Renderer(self._device)
+        r = self._renderer
+        w, h = self.res
+        frame_dt = float(np.float32(1.0) / np.float32(frame_rate))
+        hist = r.temporal_create(w, h)
+        n = 0
+        try:
+            r.upload_scene(world, camera)
+            for k in frames:
+                start = np.float32(k) * np.float32(frame_dt)
+                time_range = (float(start), float(start + np.float32(shutter)))
+                inputs = FrameInputs(w, h, samples, integrator, filt, k)
+                planes = r.render_host(inputs, tile_size, integrator, time_range, moments=True)
+                self.last_stats = r.stats()
+                self.spp = inputs.spp
+                g_inputs = FrameInputs(w, h, min(samples, ALBEDO_SAMPLES), integrator, filt, k)
+                albedo = None
+                if "albedo" in self.channel_kinds:
+                    motion, albedo = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, albedo=True)
+                else:
+                    motion = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt)
+                blend, moments, scale = r.temporal_push(hist, planes, planes["moments"], motion, reset=(n == 0), **t_kw)
+                guides = {"color": blend["color"], "background": blend["background"], "alpha": planes["alpha"], "normal": planes["normal"]}
+                out = r.denoise(w, h, guides, iterations, albedo=None if albedo is None else albedo.reshape(-1), moments=moments,
+                                spp=inputs.spp, var_scale=scale)
+                self.channels = {"color": out["color"].reshape(h, w, 3), "background": out["background"].reshape(h, w, 3),
+                                 "alpha": planes["alpha"].reshape(h, w), "normal": planes["normal"].reshape(h, w, 3)}
+                if albedo is not None:
+                    self.channels["albedo"] = albedo
+                if "motion" in self.channel_kinds:
+                    self.channels["motion"] = motion
+                self.progressive_epoch += 1
+                n += 1
+                if on_frame is not None:
+                    on_frame(self)
+        finally:
+            hist.close()
+        return n
+
     def save_to(self, write_channels, output_folder, base_name, transparent_background=False):
         """film.rs:205-377.  Same channel semantics and file names as the reference; the pixel arithmetic runs on the
         device (`rayn_b200_film_postprocess`), the PNG encoding stays host I/O (PIL)."""
@@ -519,8 +653,8 @@ class Film:
         flat = {k: np.ascontiguousarray(v, np.float32).reshape(-1) for k, v in self.channels.items()}
         written = []
         for kind in write_channels:
-            if kind == "moments":
-                raise ValueError("the moments channel is not an image: read Film.channels[\"moments\"]")
+            if kind in ("moments", "motion"):
+                raise ValueError(f"the {kind} channel is not an image: read Film.channels[\"{kind}\"]")
             if kind == "color":
                 if transparent_background and "color" in flat and "alpha" in flat:
                     mode, pil = L.POST_COLOR_ALPHA, "RGBA"
