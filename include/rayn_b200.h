@@ -389,6 +389,32 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, fl
 int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* frame, float frame_dt, float* motion /* [4*W*H] */,
                                 float* albedo /* [3*W*H] or NULL */, int32_t space);
 
+/* ---- screen-space motion against the previous frame's scene: animation that is not one linear scene ------------------------
+ * rayn_b200_render_motion measures motion by running the uploaded scene backwards, which is exact only when one upload
+ * describes the whole sequence.  A host that uploads a new scene per frame (curved camera paths, closures sampled per frame,
+ * an interactive camera) passes here the scene `prev` that frame k-1 was rendered with.  The call reads only prev->camera
+ * and prev->hitables[j].kind, .center and .center_velocity.  Everything is rayn_b200_render_motion's statement (same rays,
+ * fold, tau, validity, records and resolve; albedo as there), except the previous position and projection:
+ *   P' = P + (c_prev_j(tau - frame_dt) - c_j(tau))   for a hit on sphere hitable j, each operation rounded on its own, with
+ *        c_j(t) = seq(center, center_velocity, t) of the uploaded hitable and c_prev_j that of prev's, each formed as the
+ *        extend stage forms a sphere centre: base + v*t per component (product, then sum, each rounded), or the base itself
+ *        if v is zero; tau - frame_dt is rounded once and used for both the centre and the camera;
+ *   P' = P   for an SDF hit (there is no SDF motion), and for a sphere whose velocity is zero in both scenes and whose centres
+ *        are equal bit for bit;
+ *   (px0, py0, z_prev) = proj(P', tau - frame_dt) with prev->camera in place of the scene camera: its origin, at and up
+ *        evaluated at tau - frame_dt as camera_ray does, and its own half_size / full_size, so a zoom between frames
+ *        reprojects correctly; (px1, py1, z) = proj(P, tau) with the uploaded camera, as in rayn_b200_render_motion.
+ * Identity (tested): if prev describes the uploaded scene and no sphere moves, the plane equals rayn_b200_render_motion's bit
+ * for bit, since both projections are then the same function of the same operands.  A moving sphere whose linear parameters
+ * are unchanged still moves: its hits differ from rayn_b200_render_motion's only by rounding (c(tau - frame_dt) - c(tau)
+ * against -v*frame_dt).
+ * RAYN_ERR_INVALID_ARG: prev NULL, prev->hitables NULL, a non-finite frame_dt, prev->n_hitables different from the uploaded
+ * scene's, a hitable kind that differs, or a camera kind that differs (a cut to another camera type is a history reset, not
+ * motion).  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; stats and graph rules are rayn_b200_render_motion's
+ * (k_motion_paths_prev counts under RAYN_K_NORMALS).                                                                         */
+int32_t rayn_b200_render_motion_prev(RaynContext* ctx, const RaynFrameDesc* frame, float frame_dt, const RaynSceneDesc* prev,
+                                     float* motion /* [4*W*H] */, float* albedo /* [3*W*H] or NULL */, int32_t space);
+
 /* ---- multi-GPU: film tiles shard across GPUs, NCCL only for the final film gather -------------------------
  * The reference's only parallelism is one rayon task per tile over shared read-only state (film.rs:640-649); the
  * multi-GPU form of that is one context per GPU, each rendering the tiles `(tile_x + tile_y) % world == rank`

@@ -168,6 +168,7 @@ SYMBOLS = {
     "rayn_b200_film_denoise_variance": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), f32, C.c_void_p, i32,
                                               i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_render_motion": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), f32, C.c_void_p, C.c_void_p, i32]),
+    "rayn_b200_render_motion_prev": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), f32, C.POINTER(RaynSceneDesc), C.c_void_p, C.c_void_p, i32]),
     "rayn_b200_film_denoise_variance_scaled": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), C.c_void_p, f32,
                                                      C.c_void_p, i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
     "rayn_b200_temporal_create": (i32, [C.c_void_p, i32, i32, C.POINTER(C.c_void_p)]),

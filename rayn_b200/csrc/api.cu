@@ -101,6 +101,7 @@ struct RaynContext {
   unsigned char* d_post = nullptr;
   size_t cap_post = 0;
   unsigned long long* d_kat = nullptr;
+  DevPrev* d_prev = nullptr;  // rayn_b200_render_motion_prev's previous scene, allocated by its first call
   RaynStats stats;
   bool qlog_enabled = false;
   std::vector<int32_t> qlog;
@@ -403,6 +404,7 @@ void rayn_b200_destroy(RaynContext* ctx) {
   cudaFree(ctx->d_post);
   cudaFree(ctx->d_s1), cudaFree(ctx->d_s2), cudaFree(ctx->d_scr), cudaFree(ctx->d_fis), cudaFree(ctx->d_planes);
   cudaFree(ctx->d_moments);
+  cudaFree(ctx->d_prev);
   for (auto& t : ctx->timed) cudaEventDestroy(t.a), cudaEventDestroy(t.b);
   if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
   cudaEventDestroy(ctx->ev0), cudaEventDestroy(ctx->ev1);
@@ -1250,15 +1252,39 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float*
   return render_finish(ctx);
 }
 
-// The first-hit motion plane and optionally the albedo plane (statement in include/rayn_b200.h): the albedo pass's job with
-// k_motion_paths and k_motion_resolve (rt_motion.cuh), and k_albedo_resolve on the same per-path albedos.  Never captured.
-int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, float* motion, float* albedo, int32_t space) {
-  int32_t rc = job_ready(ctx, "render_motion");
+// The first-hit motion plane and optionally the albedo plane (statements in include/rayn_b200.h): the albedo pass's job with
+// k_motion_paths (prev == NULL) or k_motion_paths_prev and k_motion_resolve (rt_motion.cuh), and k_albedo_resolve on the same
+// per-path albedos.  Never captured.
+static int32_t motion_job(RaynContext* ctx, const char* name, const RaynFrameDesc* f, float frame_dt, bool use_prev,
+                          const RaynSceneDesc* prev, float* motion, float* albedo, int32_t space) {
+  int32_t rc = job_ready(ctx, name);
   if (rc) return rc;
   if (!f || !motion) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/motion is NULL");
-  if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_motion: bad memory space %d", space);
-  if (!isfinite(frame_dt)) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_motion: frame_dt %g is not finite", frame_dt);
-  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_motion: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
+  if (use_prev && !prev) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev is NULL", name);
+  if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: bad memory space %d", name, space);
+  if (!isfinite(frame_dt)) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: frame_dt %g is not finite", name, frame_dt);
+  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "%s: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)", name);
+  DevPrev dp;
+  if (prev) {
+    const DevScene& sc = ctx->scene;
+    if (prev->n_hitables != sc.n_hit)
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev has %d hitables, the uploaded scene %d", name, prev->n_hitables, sc.n_hit);
+    if (!prev->hitables) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev->hitables is NULL", name);
+    if (prev->camera.kind != sc.cam.kind)
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev camera kind %d differs from the uploaded %d (a cut is a reset, not motion)", name,
+                  prev->camera.kind, sc.cam.kind);
+    memset(&dp, 0, sizeof dp);
+    dp.cam = prev->camera;
+    for (int j = 0; j < sc.n_hit; ++j) {
+      const RaynHitable &p = prev->hitables[j], &h = sc.hit[j];
+      if (p.kind != h.kind) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev hitable %d has kind %d, the uploaded one %d", name, j, p.kind, h.kind);
+      memcpy(dp.center[j], p.center, sizeof dp.center[j]);
+      memcpy(dp.velocity[j], p.center_velocity, sizeof dp.velocity[j]);
+      const bool zero_v = !(p.center_velocity[0] != 0.0f || p.center_velocity[1] != 0.0f || p.center_velocity[2] != 0.0f) &&
+                          !(h.center_velocity[0] != 0.0f || h.center_velocity[1] != 0.0f || h.center_velocity[2] != 0.0f);
+      if (h.kind == RAYN_HITABLE_SPHERE && zero_v && memcmp(p.center, h.center, sizeof h.center) == 0) dp.still |= 1u << j;
+    }
+  }
   Job J;
   if ((rc = job_begin(ctx, f, nullptr, false, space, &J))) return rc;
   const DevFrame& fr = J.P.fr;
@@ -1270,6 +1296,10 @@ int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float 
     CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 7));
     dm_ = ctx->d_planes, da = albedo ? ctx->d_planes + 4 * npx : nullptr;
   }
+  if (prev) {  // pageable source: the copy has left dp when cudaMemcpyAsync returns
+    if (!ctx->d_prev) CU(cudaMalloc(&ctx->d_prev, sizeof(DevPrev)));
+    CU(cudaMemcpyAsync(ctx->d_prev, &dp, sizeof dp, cudaMemcpyHostToDevice, st));
+  }
   k_motion_clear<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>((long long)npx, dm_);  // pixels outside the tile grid
   if (da) CU(cudaMemsetAsync(da, 0, npx * 3 * sizeof(float), st));
   const Thr thr = make_thr(ctx->scene.cam, 0);
@@ -1280,7 +1310,11 @@ int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float 
     if ((rc = extend_enqueue(ctx, J, thr))) return rc;
     const dim3 gp(paths_grid.x, pb.n_tiles), gr(pix_grid.x, pb.n_tiles);
     timed_begin(ctx, RAYN_K_NORMALS);
-    if (da)
+    if (prev && da)
+      k_motion_paths_prev<true><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt, ctx->d_prev);
+    else if (prev)
+      k_motion_paths_prev<false><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt, ctx->d_prev);
+    else if (da)
       k_motion_paths<true><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
     else
       k_motion_paths<false><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
@@ -1301,6 +1335,15 @@ int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float 
     }
   }
   return render_finish(ctx);
+}
+
+int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, float* motion, float* albedo, int32_t space) {
+  return motion_job(ctx, "render_motion", f, frame_dt, false, nullptr, motion, albedo, space);
+}
+
+int32_t rayn_b200_render_motion_prev(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, const RaynSceneDesc* prev, float* motion,
+                                     float* albedo, int32_t space) {
+  return motion_job(ctx, "render_motion_prev", f, frame_dt, true, prev, motion, albedo, space);
 }
 
 int32_t rayn_b200_sync(RaynContext* ctx) {

@@ -5,10 +5,22 @@
 //                     path of a pass buffer that is idle here (PassBufs::rad, which only the shading kernels read); with an
 //                     albedo plane, also k_albedo_paths's value into PassBufs::nrm, so one march serves both guides;
 //   k_motion_resolve  one thread per pixel: the sequential mean over the pixel's valid samples, in sample order.
+// rayn_b200_render_motion_prev runs k_motion_paths_prev instead of k_motion_paths: the same body with the previous frame's
+// camera and sphere centres (DevPrev) in place of the current scene run backwards.
 #pragma once
 #include "rt_albedo.cuh"
 
 namespace rt {
+
+// What rayn_b200_render_motion_prev reads of the previous frame's scene, in a 516-byte device buffer the call writes.  It is
+// not a kernel parameter: k_motion_paths's block (DevScene, DevFrame, PassBufs, frame_dt) is 3844 bytes, and this would take
+// it past the 4 KB that rt_kernels.cuh's scene limits are sized for.
+struct DevPrev {
+  RaynCamera cam;
+  float center[RAYN_MAX_HITABLES][3];
+  float velocity[RAYN_MAX_HITABLES][3];
+  uint32_t still;  // bit j: hitable j is a sphere with a zero velocity in both scenes and the same centre bit for bit (P' = P)
+};
 
 // Film position (px, py) in pixels and view depth z of point X for camera c at `time`: the inverse of camera_ray's
 // pixel -> (u, v) map (the thin lens through its lens centre).  The one projection both times go through.
@@ -35,8 +47,9 @@ RT_D void camera_project(const RaynCamera& c, int W, int H, f3 X, float time, fl
 }
 
 // Path g's record (dx, dy, z, z_prev), or (0, 0, NaN, NaN) for an invalid sample; with albedo, a_s as k_albedo_paths.
-template <bool kAlb>
-__global__ void __launch_bounds__(256) k_motion_paths(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb, float frame_dt) {
+// kPrev: the previous projection and a sphere hit's previous position come from *pv (rayn_b200_render_motion_prev).
+template <bool kAlb, bool kPrev>
+RT_D void motion_path(const DevScene& sc, const DevFrame& fr, const PassBufs& pb, float frame_dt, const DevPrev* __restrict__ pv) {
   const int ts = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const TileGeom tg = tile_geom(fr, pb.tile_ids[ts]);
@@ -52,10 +65,15 @@ __global__ void __launch_bounds__(256) k_motion_paths(const __grid_constant__ De
     // lane 0 of the camera packet: its o_time.w is the time raygen evaluated the camera at (depth 0: nothing moved it)
     const float tau = (i & 3) ? pb.o_time[g - (i & 3)].w : o4.w;
     f3 Pp = P;
-    if (sphere_moves(h)) Pp = P - ld3(h.center_velocity) * frame_dt;
+    if constexpr (kPrev) {  // P + (c_prev(tau - dt) - c(tau)), both centres as the extend stage forms them
+      if (h.kind == RAYN_HITABLE_SPHERE && !((pv->still >> key) & 1u))
+        Pp = P + (seq3(pv->center[key], pv->velocity[key], tau - frame_dt) - sphere_center(h, tau));
+    } else {
+      if (sphere_moves(h)) Pp = P - ld3(h.center_velocity) * frame_dt;
+    }
     float px1, py1, z1, px0, py0, z0;
     camera_project(sc.cam, fr.W, fr.H, P, tau, &px1, &py1, &z1);
-    camera_project(sc.cam, fr.W, fr.H, Pp, tau - frame_dt, &px0, &py0, &z0);
+    camera_project(kPrev ? pv->cam : sc.cam, fr.W, fr.H, Pp, tau - frame_dt, &px0, &py0, &z0);
     if (sc.cam.kind == RAYN_CAMERA_ORTHOGRAPHIC || (z1 > 0.0f && z0 > 0.0f)) rec = make_float4(px0 - px1, py0 - py1, z1, z0);
     if (kAlb) {
       const RaynMaterial& mat = sc.mat[h.material];
@@ -72,6 +90,18 @@ __global__ void __launch_bounds__(256) k_motion_paths(const __grid_constant__ De
   }
   pb.rad[g] = rec;
   if (kAlb) pb.nrm[g] = make_float4(a.x, a.y, a.z, 0.0f);
+}
+
+template <bool kAlb>
+__global__ void __launch_bounds__(256) k_motion_paths(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb, float frame_dt) {
+  motion_path<kAlb, false>(sc, fr, pb, frame_dt, nullptr);
+}
+
+// rayn_b200_render_motion_prev; its own kernel, so that k_motion_paths's parameter block and code stay as they are
+template <bool kAlb>
+__global__ void __launch_bounds__(256) k_motion_paths_prev(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb, float frame_dt,
+                                                           const DevPrev* __restrict__ pv) {
+  motion_path<kAlb, true>(sc, fr, pb, frame_dt, pv);
 }
 
 // motion[4 pix + k] = (((+0 + r_a[k]) + r_b[k]) + ...) / (float)n over the pixel's valid samples (z not NaN), sample order;

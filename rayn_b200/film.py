@@ -209,14 +209,18 @@ class Renderer:
     def ctx(self):
         return self._ctx
 
-    def upload_scene(self, world, camera):
-        """Uploads the scene, then its orbit-trap albedos (OrbitTrapAlbedo materials), if it has any."""
-        desc, keep = world.flatten(camera)
+    def upload_scene(self, world, camera, time_range=None):
+        """Uploads the scene, then its orbit-trap albedos (OrbitTrapAlbedo materials), if it has any.  time_range: the (t0, t1)
+        of the renders that follow, required if the scene has closure parameters (each is uploaded as its chord over it,
+        Linear.chord).  Returns World.flatten's (RaynSceneDesc, keepalive), e.g. the `prev` of the next frame's
+        render_motion."""
+        desc, keep = world.flatten(camera, time_range)
         self._keep = (desc, keep)
         L.check(self._lib.rayn_b200_upload_scene(self._ctx, C.byref(desc)), self._ctx)
         traps = world.albedo_traps()
         if traps:
             self.set_albedo_traps(traps)
+        return desc, keep
 
     def set_albedo_traps(self, traps):
         """Replaces the orbit-trap list of the uploaded scene (include/rayn_b200.h: rayn_b200_set_albedo_traps): a list of
@@ -264,17 +268,23 @@ class Renderer:
         L.check(self._lib.rayn_b200_render_albedo(self._ctx, C.byref(f), out.ctypes.data, L.MEM_HOST), self._ctx)
         return out.reshape(h, w, 3)
 
-    def render_motion(self, inputs, tile_size, integrator, time_range, frame_dt, albedo=False):
+    def render_motion(self, inputs, tile_size, integrator, time_range, frame_dt, albedo=False, prev=None):
         """First-hit motion plane of the uploaded scene (include/rayn_b200.h: rayn_b200_render_motion) for host FrameInputs:
-        float32 [H, W, 4] (dx, dy, z, z_prev); albedo=True: (motion, render_albedo's [H, W, 3] plane from the same pass)."""
+        float32 [H, W, 4] (dx, dy, z, z_prev); albedo=True: (motion, render_albedo's [H, W, 3] plane from the same pass).
+        prev: the RaynSceneDesc the previous frame was rendered with (World.flatten's or upload_scene's, its keepalive still
+        held): the motion against that scene instead of the uploaded one run backwards (rayn_b200_render_motion_prev)."""
         w, h = inputs.width, inputs.height
         out = np.zeros(4 * w * h, np.float32)
         alb = np.zeros(3 * w * h, np.float32) if albedo else None
         ptrs = tuple(a.ctypes.data for a in inputs.arrays())
         f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST,
                             sets=(inputs.sets_1d, inputs.sets_2d))
-        L.check(self._lib.rayn_b200_render_motion(self._ctx, C.byref(f), float(frame_dt), out.ctypes.data,
-                                                  None if alb is None else alb.ctypes.data, L.MEM_HOST), self._ctx)
+        a_ptr = None if alb is None else alb.ctypes.data
+        if prev is None:
+            L.check(self._lib.rayn_b200_render_motion(self._ctx, C.byref(f), float(frame_dt), out.ctypes.data, a_ptr, L.MEM_HOST), self._ctx)
+        else:
+            L.check(self._lib.rayn_b200_render_motion_prev(self._ctx, C.byref(f), float(frame_dt), C.byref(prev), out.ctypes.data, a_ptr,
+                                                           L.MEM_HOST), self._ctx)
         return (out.reshape(h, w, 4), alb.reshape(h, w, 3)) if albedo else out.reshape(h, w, 4)
 
     def temporal_create(self, width, height):
@@ -505,7 +515,7 @@ class Film:
             self._renderer = Renderer(self._device)
         w, h = self.res
         inputs = FrameInputs(w, h, samples, integrator, filt, frame)
-        self._renderer.upload_scene(world, camera)
+        self._renderer.upload_scene(world, camera, time_range)
         planes = self._renderer.render_host(inputs, tile_size, integrator, time_range, moments="moments" in self.channel_kinds)
         self.last_stats = self._renderer.stats()
         self.spp = inputs.spp
@@ -545,7 +555,7 @@ class Film:
         w, h = self.res
         spp = 4 * samples_per_round
         sets = (1 + integrator.requested_1d_sample_sets(), 2 + integrator.requested_2d_sample_sets())  # film.rs:431-432
-        r.upload_scene(world, camera)
+        r.upload_scene(world, camera, time_range)
         dev = torch.device("cuda", r.device)
         s1 = torch.empty(spp * sets[0], dtype=torch.float32, device=dev)
         s2 = torch.empty(2 * spp * sets[1], dtype=torch.float32, device=dev)
@@ -595,7 +605,12 @@ class Film:
         4 * min(samples, ALBEDO_SAMPLES) samples, as render_frame_into's); the push into a film history (reset on the first
         frame); the variance-guided denoise of the blend with its per-pixel variance scale; then on_frame(film).  The
         temporal parameters default to TEMPORAL_DEFAULTS.  self.channels holds the denoised colour and background and the
-        frame's alpha, normal, albedo and motion planes (the ones the Film has).  Returns the number of frames."""
+        frame's alpha, normal, albedo and motion planes (the ones the Film has).  Returns the number of frames.
+
+        A world with closure parameters (World.has_closures: a sphere on a curved path, an orbiting camera) is uploaded
+        before every frame as its chord over that frame's time range, and every frame after the first measures its motion
+        against the scene the previous frame was rendered with (Renderer.render_motion(prev=...)).  Any other world is
+        uploaded once and its motion is the uploaded scene run backwards."""
         if "moments" in self.channel_kinds:
             raise ValueError("render_sequence consumes the moments of every frame: create the Film without \"moments\"")
         for k in ("color", "background", "alpha", "normal"):
@@ -603,28 +618,33 @@ class Film:
                 raise ValueError(f"render_sequence needs the {k} channel")
         t_kw = {k: float(TEMPORAL_DEFAULTS[k] if v is None else v)
                 for k, v in dict(alpha_min=alpha_min, sigma_depth=sigma_depth, normal_cos=normal_cos).items()}
+        animated = world.has_closures(camera)
         if self._renderer is None:
             self._renderer = Renderer(self._device)
         r = self._renderer
         w, h = self.res
         frame_dt = float(np.float32(1.0) / np.float32(frame_rate))
         hist = r.temporal_create(w, h)
-        n = 0
+        n, prev, scene = 0, None, None
         try:
-            r.upload_scene(world, camera)
+            if not animated:
+                r.upload_scene(world, camera)
             for k in frames:
                 start = np.float32(k) * np.float32(frame_dt)
                 time_range = (float(start), float(start + np.float32(shutter)))
+                if animated:
+                    prev, scene = scene, r.upload_scene(world, camera, time_range)
                 inputs = FrameInputs(w, h, samples, integrator, filt, k)
                 planes = r.render_host(inputs, tile_size, integrator, time_range, moments=True)
                 self.last_stats = r.stats()
                 self.spp = inputs.spp
                 g_inputs = FrameInputs(w, h, min(samples, ALBEDO_SAMPLES), integrator, filt, k)
                 albedo = None
+                p_desc = None if prev is None else prev[0]  # None on the first frame, which resets the history
                 if "albedo" in self.channel_kinds:
-                    motion, albedo = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, albedo=True)
+                    motion, albedo = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, albedo=True, prev=p_desc)
                 else:
-                    motion = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt)
+                    motion = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, prev=p_desc)
                 blend, moments, scale = r.temporal_push(hist, planes, planes["moments"], motion, reset=(n == 0), **t_kw)
                 guides = {"color": blend["color"], "background": blend["background"], "alpha": planes["alpha"], "normal": planes["normal"]}
                 out = r.denoise(w, h, guides, iterations, albedo=None if albedo is None else albedo.reshape(-1), moments=moments,

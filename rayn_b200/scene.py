@@ -71,18 +71,50 @@ def _arr(x):
 
 class Linear:
     """A `Sequenced` parameter that is linear in time: value(t) = base + velocity * t.  Stands for the closure
-    `move |t| base + velocity * t` a rayn scene would pass (animation.rs:55-68); arbitrary closures cannot cross a C ABI.
-    Like every closure-backed WSequenced it is evaluated at lane 0's time for a whole 4-lane packet (animation.rs:62-67)."""
+    `move |t| base + velocity * t` a rayn scene would pass (animation.rs:55-68).  Like every closure-backed WSequenced it is
+    evaluated at lane 0's time for a whole 4-lane packet (animation.rs:62-67).
+
+    Any other closure `f(t) -> Vec3` (or a 3-sequence) may be passed where a scene takes a Linear, but only linear-in-time
+    parameters cross the C ABI: each render uploads the closure's chord over its time range (Linear.chord)."""
 
     def __init__(self, base, velocity):
         self.base, self.velocity = base, velocity
 
+    @staticmethod
+    def chord(f, t0, t1):
+        """The Linear that equals closure f at the shutter ends t0 and t1 (each rounded to float32 first, as the renderer
+        takes them): velocity = (f(t1) - f(t0)) / (t1 - t0) and base = f(t0) - velocity * t0, computed in float64 and then
+        rounded to float32; for t1 == t0, velocity 0 and base f(t0).  An approximation of rayn, which evaluates the closure at
+        every packet's lane-0 time: the chord is exact at t0 and t1 only (up to the float32 rounding of base, velocity and
+        the renderer's base + velocity * t), and in between it is the straight line between them."""
+        t0, t1 = float(np.float32(t0)), float(np.float32(t1))
+        a = np.asarray(_arr(f(t0)), np.float64)
+        if t1 == t0:
+            return Linear(a.astype(np.float32), np.zeros(3, np.float32))
+        v = (np.asarray(_arr(f(t1)), np.float64) - a) / (t1 - t0)
+        return Linear((a - v * t0).astype(np.float32), v.astype(np.float32))
+
+
+def _is_closure(x):
+    return callable(x) and not isinstance(x, (Vec3, Linear))
+
 
 def _seq(x):
-    """-> (base[3], velocity[3]) for a constant or Linear Vec3 parameter."""
+    """-> (base[3], velocity[3]) for a constant or Linear Vec3 parameter; a closure is kept as it is (see _at)."""
+    if _is_closure(x):
+        return x
     if isinstance(x, Linear):
         return _arr(x.base), _arr(x.velocity)
     return _arr(x), np.zeros(3, np.float32)
+
+
+def _at(p, time_range):
+    """-> (base[3], velocity[3]) of a parameter _seq made, for one render over time_range: a closure's chord there."""
+    if not _is_closure(p):
+        return p
+    if time_range is None:
+        raise ValueError("a scene with closure parameters needs the render's time_range to flatten (Linear.chord)")
+    return _seq(Linear.chord(p, time_range[0], time_range[1]))
 
 
 # ---- materials (material.rs) ---------------------------------------------------------------
@@ -186,16 +218,23 @@ class MaterialStore:  # material.rs:58-73
 
 
 # ---- hitables (sphere.rs, sdf.rs) --------------------------------------------------------------
-class Sphere:  # sphere.rs:14-20 (centre: constant or Linear)
+class Sphere:  # sphere.rs:14-20 (centre: constant, Linear or a closure f(t) -> Vec3)
     def __init__(self, center, radius, material):
-        (self.center, self.center_velocity), self.radius, self.material = _seq(center), f32(radius), int(material)
+        # a closure centre is kept as it is, with center_velocity None
+        self.center, self.center_velocity = (center, None) if _is_closure(center) else _seq(center)
+        self.radius, self.material = f32(radius), int(material)
 
-    def flatten(self):
+    def has_closures(self):
+        return self.center_velocity is None
+
+    def flatten(self, time_range=None):
+        """time_range: the render's (t0, t1), needed if the centre is a closure (its chord there is uploaded)"""
+        center, velocity = _at(self.center, time_range) if self.has_closures() else (self.center, self.center_velocity)
         h = L.RaynHitable()
         h.kind = L.HITABLE_SPHERE
         h.material = self.material
-        h.center[:] = self.center.tolist()
-        h.center_velocity[:] = self.center_velocity.tolist()
+        h.center[:] = center.tolist()
+        h.center_velocity[:] = velocity.tolist()
         h.radius = float(self.radius)
         return h
 
@@ -227,7 +266,11 @@ class TracedSDF:  # sdf.rs:12-21
     def __init__(self, sdf, material):
         self.sdf, self.material = sdf, int(material)
 
-    def flatten(self):
+    def has_closures(self):
+        return False
+
+    def flatten(self, time_range=None):
+        """time_range is not used: an SDF has no time-varying parameter"""
         h = L.RaynHitable()
         h.material = self.material
         s = self.sdf
@@ -273,12 +316,22 @@ class SphereLight:  # light.rs:27-34
 
 
 # ---- cameras (camera.rs) ----------------------------------------------------------------------------
-def _store_seq(c, origin, at, up, focus=None):
+def _store_seq(c, time_range, origin, at, up, focus=None):
+    origin, at, up = _at(origin, time_range), _at(at, time_range), _at(up, time_range)
     c.origin[:], c.origin_velocity[:] = origin[0].tolist(), origin[1].tolist()
     c.at[:], c.at_velocity[:] = at[0].tolist(), at[1].tolist()
     c.up[:], c.up_velocity[:] = up[0].tolist(), up[1].tolist()
     if focus is not None:
+        focus = _at(focus, time_range)
         c.focus[:], c.focus_velocity[:] = focus[0].tolist(), focus[1].tolist()
+
+
+class _Camera:
+    """The sequenced parameters of a camera (origin, at, up and a thin lens's focus): constants, Linear or closures; a
+    closure's chord over the render's time_range is what flatten(time_range) stores."""
+
+    def has_closures(self):
+        return any(_is_closure(p) for p in (self.origin, self.at, self.up, getattr(self, "focus", None)))
 
 
 def _fov_half(resolution, vfov):
@@ -290,23 +343,23 @@ def _fov_half(resolution, vfov):
     return f32(half_width), f32(half_height)
 
 
-class PinholeCamera:  # camera.rs:52-72
+class PinholeCamera(_Camera):  # camera.rs:52-72
     def __init__(self, resolution, vfov, origin, at, up):
         self.res = (f32(resolution[0]), f32(resolution[1]))
         self.half_width, self.half_height = _fov_half(self.res, vfov)
         self.half_pixel_size = self.half_height / self.res[1]
         self.origin, self.at, self.up = _seq(origin), _seq(at), _seq(up)
 
-    def flatten(self):
+    def flatten(self, time_range=None):
         c = L.RaynCamera()
         c.kind = L.CAMERA_PINHOLE
         c.half_size[:] = [float(self.half_width), float(self.half_height)]
         c.half_pixel_size = float(self.half_pixel_size)
-        _store_seq(c, self.origin, self.at, self.up)
+        _store_seq(c, time_range, self.origin, self.at, self.up)
         return c
 
 
-class ThinLensCamera:  # camera.rs:133-157
+class ThinLensCamera(_Camera):  # camera.rs:133-157
     def __init__(self, resolution, vfov, aperture, origin, at, up, focus):
         self.res = (f32(resolution[0]), f32(resolution[1]))
         self.half_width, self.half_height = _fov_half(self.res, vfov)
@@ -314,18 +367,18 @@ class ThinLensCamera:  # camera.rs:133-157
         self.aperture, self.aperture_rate = (f32(aperture.base), f32(aperture.velocity)) if isinstance(aperture, Linear) else (f32(aperture), f32(0.0))
         self.origin, self.at, self.up, self.focus = _seq(origin), _seq(at), _seq(up), _seq(focus)
 
-    def flatten(self):
+    def flatten(self, time_range=None):
         c = L.RaynCamera()
         c.kind = L.CAMERA_THINLENS
         c.half_size[:] = [float(self.half_width), float(self.half_height)]
         c.half_pixel_size = float(self.half_pixel_size)
-        _store_seq(c, self.origin, self.at, self.up, self.focus)
+        _store_seq(c, time_range, self.origin, self.at, self.up, self.focus)
         c.aperture = float(self.aperture)
         c.aperture_rate = float(self.aperture_rate)
         return c
 
 
-class OrthographicCamera:  # camera.rs:227-241
+class OrthographicCamera(_Camera):  # camera.rs:227-241
     def __init__(self, resolution, vertical_size, origin, at, up):
         self.res = (f32(resolution[0]), f32(resolution[1]))
         aspect = self.res[0] / self.res[1]
@@ -333,13 +386,13 @@ class OrthographicCamera:  # camera.rs:227-241
         self.pixel_size = f32(vertical_size) / self.res[1]
         self.origin, self.at, self.up = _seq(origin), _seq(at), _seq(up)
 
-    def flatten(self):
+    def flatten(self, time_range=None):
         c = L.RaynCamera()
         c.kind = L.CAMERA_ORTHOGRAPHIC
         c.half_size[:] = [float(self.size[0] / f32(2.0)), float(self.size[1] / f32(2.0))]
         c.full_size[:] = [float(self.size[0]), float(self.size[1])]
         c.half_pixel_size = float(self.pixel_size / f32(2.0))
-        _store_seq(c, self.origin, self.at, self.up)
+        _store_seq(c, time_range, self.origin, self.at, self.up)
         return c
 
 
@@ -374,17 +427,23 @@ class World:  # world.rs:7-13
         self.volume_params = volume_params
         self.consts = consts or RenderConsts()
 
-    def flatten(self, camera_handle):
-        """-> (RaynSceneDesc, keepalive).  Order of hitables / materials / lights is preserved."""
+    def has_closures(self, camera_handle):
+        """True if a sphere centre or a sequenced parameter of the camera is a closure f(t) -> Vec3 (Linear.chord)."""
+        return self.cameras.get(camera_handle).has_closures() or any(h.has_closures() for h in self.hitables.items)
+
+    def flatten(self, camera_handle, time_range=None):
+        """-> (RaynSceneDesc, keepalive).  Order of hitables / materials / lights is preserved.  time_range: the render's
+        (t0, t1); a closure parameter is uploaded as its chord over it (Linear.chord), and without it raises ValueError.
+        A scene without closures flattens the same whatever time_range."""
         nh, nm, nl = len(self.hitables.items), len(self.materials.items), len(self.lights)
-        hit = (L.RaynHitable * max(nh, 1))(*[h.flatten() for h in self.hitables.items])
+        hit = (L.RaynHitable * max(nh, 1))(*[h.flatten(time_range) for h in self.hitables.items])
         mat = (L.RaynMaterial * max(nm, 1))(*[m.flatten() for m in self.materials.items])
         lig = (L.RaynLight * max(nl, 1))(*[l.flatten() for l in self.lights])
         d = L.RaynSceneDesc()
         d.n_hitables, d.hitables = nh, C.cast(hit, C.POINTER(L.RaynHitable))
         d.n_materials, d.materials = nm, C.cast(mat, C.POINTER(L.RaynMaterial))
         d.n_lights, d.lights = nl, C.cast(lig, C.POINTER(L.RaynLight))
-        d.camera = self.cameras.get(camera_handle).flatten()
+        d.camera = self.cameras.get(camera_handle).flatten(time_range)
         v = self.volume_params
         d.volume.has_scattering = 0 if v.coeff_scattering is None else 1
         d.volume.coeff_scattering = float(v.coeff_scattering or 0.0)
