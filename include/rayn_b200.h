@@ -555,9 +555,10 @@ int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoi
  * p = (x, y), in float, no contraction:
  *   reset = 0 and z_prev finite:  fx = (((float)x + 0.5f) + dx) - 0.5f, fy likewise; x0 = floorf(fx), y0 = floorf(fy), ax = fx - x0, ay = fy - y0;
  *     taps (x0 + i, y0 + j), j outer, i inner, in {0, 1}, weight w = (i ? ax : 1 - ax) * (j ? ay : 1 - ay).  A tap is USED if
- *     w != 0, it is inside the image (compared in float), its history n > 0, its colour and background are finite,
- *     fabsf(z_h - z_prev) <= sigma_depth * fabsf(z_prev) (so z_h is finite; |z_prev| serves orthographic views, whose z may
- *     be <= 0) and ((nx_h*nx + ny_h*ny) + nz_h*nz) >= normal_cos (n the current normal).
+ *     w != 0, it is inside the image (compared in float), its history n > 0, its colour and background are finite, z_h is
+ *     finite and fabsf(z_h - z_prev) <= sigma_depth * fabsf(z_prev) (|z_prev| serves orthographic views, whose z may be
+ *     <= 0; z_h is tested on its own because sigma_depth = +inf, or an overflowing product, would otherwise pass a history
+ *     without a hit, z_h = +inf) and ((nx_h*nx + ny_h*ny) + nz_h*nz) >= normal_cos (n the current normal).
  *     ws = sum w, and every history value X (colour, background, moments, n, s) is X_h = (sum w*X_q) / ws, sums in tap order
  *     over the used taps.  No used tap: n_h = 0.
  *   reset = 1, or z_prev not finite (a pixel without a valid hit: motion (0, 0, +inf, +inf)):  n_h = 0.
@@ -565,13 +566,19 @@ int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoi
  *   alpha == 1 (always when n_h = 0): every output is the current frame's value bit for bit, n' = n_h + 1, s' = 1;
  *   otherwise, for colour, background and both moments: x' = (1 - alpha) * x_h + alpha * x,  n' = n_h + 1,
  *     s' = ((1 - alpha) * (1 - alpha)) * s_h + alpha * alpha.
- * s' is the sum of squared blend weights: for frames with independent noise the variance of the blended pixel mean is
- * max(M' - lum(c')^2, 0) * s' / spp, exact for this exponential moving average (a cumulative mean, alpha_min -> 0 on a static
- * view, gives s' = 1/n').  The push writes c', b' to out, M' to out_moments and s' to var_scale, and stores c', b', M', n', s'
- * with the current normal and z in the history.  out may alias in (each pixel reads only its own input).  Every plane and
- * var_scale is required and in one memory space (in->space); host planes are staged and the call is synchronous, device
- * planes run asynchronously on the context's stream (rayn_b200_sync waits).  RAYN_ERR_INVALID_ARG for a NULL plane, mixed
- * spaces, or a bad desc.                                                                                                  */
+ * s' is the sum of squared blend weights, and for frames with independent noise max(M' - lum(c')^2, 0) * s' / spp is an
+ * UPPER BOUND on the variance of the blended pixel mean.  It is exact when no pixel resamples its history (integer motion,
+ * every used tap with weight 1; a cumulative mean, alpha_min -> 0 on a static view, gives s' = 1/n').  Under sub-pixel
+ * motion the bilinear taps average the independent noise of neighbouring history pixels (sum w^2 < sum w of their variance)
+ * while s_h is interpolated linearly, so the true variance is smaller: about 0.78 of the bound at 0.1 px per frame, 0.60 at
+ * 0.5 px and 0.46 at (0.5, 0.5) px, with alpha_min 0.2 (tested).  The bound holds by Minkowski's and Jensen's inequalities.
+ * The push writes c', b' to out, M' to out_moments and s' to var_scale, and stores c', b', M', n', s' with the current normal
+ * and z in the history.  out may alias in (each pixel reads only its own input).  Every plane and var_scale is required and
+ * in one memory space (in->space); host planes are staged and the call is synchronous, device planes run asynchronously on
+ * the context's stream (rayn_b200_sync waits).  RAYN_ERR_INVALID_ARG for a NULL plane, mixed spaces, or a bad desc.
+ * temporal_create: width and height in [1, 2^23] and width * height <= 2^31, else RAYN_ERR_INVALID_ARG.  Up to 2^23 every
+ * pixel centre (float)x + 0.5f is exact, so a static pixel reads its own history; beyond it x + 0.5f rounds and the push
+ * would read a neighbour's.                                                                                               */
 typedef struct RaynTemporal RaynTemporal;
 typedef struct RaynTemporalDesc {
   float alpha_min;    /* (0, 1]: the smallest blend weight of the new frame                */

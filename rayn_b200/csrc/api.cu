@@ -1901,7 +1901,9 @@ struct RaynTemporal {
 
 int32_t rayn_b200_temporal_create(RaynContext* ctx, int32_t W, int32_t H, RaynTemporal** out) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
-  if (!out || W <= 0 || H <= 0 || (int64_t)W * H > ((int64_t)1 << 31)) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_create: bad argument");
+  // W, H <= 2^23: every pixel centre (float)x + 0.5f of the push is then exact
+  if (!out || W <= 0 || H <= 0 || W > (1 << 23) || H > (1 << 23) || (int64_t)W * H > ((int64_t)1 << 31))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_create: bad argument");
   *out = nullptr;
   CU(cudaSetDevice(ctx->device));
   RaynTemporal* t = new RaynTemporal();

@@ -51,7 +51,9 @@ __global__ void __launch_bounds__(256) k_temporal(int W, int H, RaynTemporalDesc
         const float c0 = hin[TH_C * npx + q], c1 = hin[(TH_C + 1) * npx + q], c2 = hin[(TH_C + 2) * npx + q];
         const float b0 = hin[TH_B * npx + q], b1 = hin[(TH_B + 1) * npx + q], b2 = hin[(TH_B + 2) * npx + q];
         if (!(isfinite(c0) && isfinite(c1) && isfinite(c2) && isfinite(b0) && isfinite(b1) && isfinite(b2))) continue;
-        if (!(fabsf(hin[TH_Z * npx + q] - zp) <= d.sigma_depth * fabsf(zp))) continue;  // false for a non-finite z_h
+        // z_h must be finite on its own: with sigma_depth * |z_prev| = +inf the comparison would pass a sky history (z_h = +inf)
+        const float zh = hin[TH_Z * npx + q];
+        if (!(isfinite(zh) && fabsf(zh - zp) <= d.sigma_depth * fabsf(zp))) continue;
         const float nd = (hin[TH_N * npx + q] * nx + hin[(TH_N + 1) * npx + q] * ny) + hin[(TH_N + 2) * npx + q] * nz;
         if (!(nd >= d.normal_cos)) continue;
         ws += w;

@@ -54,7 +54,7 @@ int32_t rayn_oracle_film_denoise_variance_scaled(const RaynDenoiseDesc* d, float
 int32_t rayn_oracle_temporal_push(int32_t W, int32_t H, const RaynTemporalDesc* d, const float* hin, float* hout, const float* c, const float* b,
                                   const float* nrm, const float* mc, const float* mb, const float* motion, float* oc, float* ob, float* omc,
                                   float* omb, float* scale) {
-  if (!d || W <= 0 || H <= 0 || !(d->alpha_min > 0.0f && d->alpha_min <= 1.0f) || !(d->sigma_depth > 0.0f) ||
+  if (!d || W <= 0 || H <= 0 || W > (1 << 23) || H > (1 << 23) || !(d->alpha_min > 0.0f && d->alpha_min <= 1.0f) || !(d->sigma_depth > 0.0f) ||
       !(d->normal_cos >= -1.0f && d->normal_cos <= 1.0f) || (d->reset != 0 && d->reset != 1))
     return RAYN_ERR_INVALID_ARG;
   const size_t npx = (size_t)W * H;

@@ -17,6 +17,7 @@ from rayn_b200.scene import OrbitTrapAlbedo
 import albedo_oracle as ao
 import denoise_oracle as dor
 import moments_oracle as mo
+import temporal_oracle as to
 from helpers import assert_bit_equal, small_config
 from test_cpu_denoise import random_film
 from test_cpu_trap import ALBEDO_HI, ALBEDO_LO, TRAP_HI, TRAP_LO, with_fractal_albedo
@@ -86,8 +87,9 @@ def moment_film(w, h, seed):
     return p, m
 
 
-def np_variance(planes, key, moments, spp, iters, sc, sn, sa, sl, albedo=None, sal=np.inf):
-    """The header's statement of rayn_b200_film_denoise_variance in numpy float32, per tap in tap order."""
+def np_variance(planes, key, moments, spp, iters, sc, sn, sa, sl, albedo=None, sal=np.inf, scale=None):
+    """The header's statement of rayn_b200_film_denoise_variance in numpy float32, per tap in tap order.  scale (float32
+    [H, W]): rayn_b200_film_denoise_variance_scaled's per-pixel variance scale of level 0."""
     vexp = np.vectorize(lambda x: dor.exp(f32(x)), otypes=[f32])
     c = np.asarray(planes[key], f32).copy()
     H, W = c.shape[:2]
@@ -96,7 +98,8 @@ def np_variance(planes, key, moments, spp, iters, sc, sn, sa, sl, albedo=None, s
     il = f32(0) if albedo is None or np.isinf(sal) else f32(1) / (f32(sal) * f32(sal))
     alb = None if albedo is None else np.asarray(albedo, f32).reshape(H, W, 3)
     l0 = lum(c)
-    v = np.fmax(np.asarray(moments, f32)[:, :, 0 if key == "color" else 1] - l0 * l0, f32(0)) / f32(spp)
+    v = np.fmax(np.asarray(moments, f32)[:, :, 0 if key == "color" else 1] - l0 * l0, f32(0))
+    v = (v if scale is None else v * np.asarray(scale, f32).reshape(H, W)) / f32(spp)
     yy, xx = np.mgrid[0:H, 0:W]
     h5, k3 = [f32(x) for x in (0.0625, 0.25, 0.375, 0.25, 0.0625)], [f32(0.25), f32(0.5), f32(0.25)]
 
@@ -157,6 +160,26 @@ def test_mirror_matches_the_numpy_statement(w, h, iters, sl, with_albedo):
     for k in ("color", "background"):
         ref = np_variance(p, k, m, 16, iters, 2.5, 0.4, 0.5, sl, alb, 0.3)
         assert_bit_equal(out[k].reshape(h, w, 3), ref, f"{k} {w}x{h} L={iters}")
+
+
+@pytest.mark.parametrize("w,h,iters,with_albedo", [(9, 7, 3, False), (13, 5, 4, True), (1, 1, 1, False)])
+def test_scaled_mirror_matches_the_numpy_statement(w, h, iters, with_albedo):
+    """rayn_b200_film_denoise_variance_scaled's mirror against the numpy statement with a per-pixel scale: random scales,
+    0, 1e-30 and 1e30 next to unit ones"""
+    p, m = moment_film(w, h, 31 + w)
+    p["color"][h // 2, w // 2, 0] = np.inf
+    rng = np.random.default_rng(w * h)
+    scale = rng.choice(np.array([0.0, 1e-30, 1e30, 1.0, 1.0], f32), (h, w))
+    scale = np.where(rng.uniform(size=(h, w)) < 0.4, rng.uniform(0.0, 3.0, (h, w)).astype(f32), scale).astype(f32)
+    alb = rng.uniform(0, 1, (h, w, 3)).astype(f32) if with_albedo else None
+    desc = denoise_desc(iters, 2.5, 0.4, 0.5)
+    rc, out = to.denoise_scaled(w, h, p, desc, 1.5, 16, m, scale, 0.3, alb)
+    assert rc == L.RAYN_OK
+    for k in ("color", "background"):
+        ref = np_variance(p, k, m, 16, iters, 2.5, 0.4, 0.5, 1.5, alb, 0.3, scale=scale)
+        assert_bit_equal(out[k].reshape(h, w, 3), ref, f"{k} {w}x{h} L={iters}")
+        if w * h > 1:  # the scale reaches the result
+            assert not np.array_equal(ref, np_variance(p, k, m, 16, iters, 2.5, 0.4, 0.5, 1.5, alb, 0.3)), k
 
 
 def test_variance_term_changes_the_result():
