@@ -1,6 +1,6 @@
 // rt_denoise.cuh — edge-avoiding a-trous wavelet filter of the film planes (Dammertz, Sewtz, Hanika, Lensch, HPG 2010).
 // The exact statement (tap order, the float arithmetic, which taps are skipped) is at rayn_b200_film_denoise in
-// include/rayn_b200.h; the CPU mirror in tests/denoise_oracle.cpp restates it and the GPU tests compare bit for bit.
+// include/rayn_b200.h; the CPU mirror in tests/film_mirror.cpp restates it and the GPU tests compare bit for bit.
 //
 // One kernel launch per level, one thread per pixel on 32x8 CTAs.  The guides are packed once into a float4
 // (nx, ny, nz, a) plane and the colour ping-pongs between two float4 planes, so every tap is two 16-byte loads that

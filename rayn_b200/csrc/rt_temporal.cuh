@@ -1,5 +1,5 @@
 // rt_temporal.cuh — temporal accumulation of a frame sequence (rayn_b200_temporal_push; the exact statement is in
-// include/rayn_b200.h, the CPU mirror in tests/temporal_oracle.cpp).
+// include/rayn_b200.h, the CPU mirror in tests/film_mirror.cpp).
 //
 // One thread per pixel.  The history is 14 planes of W*H floats (structure of arrays, so every plane access of a warp is
 // coalesced); a push reads one history and writes the other, so no thread reads a tap another thread is writing.

@@ -1,6 +1,6 @@
-"""CPU mirrors of the first-hit albedo plane (tests/albedo_oracle.cpp) and of the albedo-guided denoise
-(tests/denoise_albedo_oracle.cpp): the resolve against numpy, the alpha identity against the render oracle, the guided filter
-against the unguided mirror at sigma_albedo = +inf, albedo edges that do not mix, and the skip rules for non-finite albedo."""
+"""CPU mirrors of the first-hit albedo plane (tests/render_mirror.cpp) and of the albedo-guided denoise
+(tests/film_mirror.cpp): the resolve against numpy, the alpha identity against the render oracle, the guided filter
+against the unguided entry point at sigma_albedo = +inf, albedo edges that do not mix, and the skip rules for non-finite albedo."""
 import numpy as np
 import pytest
 
@@ -9,8 +9,7 @@ from rayn_b200 import configs
 from rayn_b200.film import denoise_desc
 from rayn_b200.scene import Dielectric, Lambertian, OrbitTrapAlbedo
 
-import albedo_oracle as ao
-import denoise_oracle as dor
+import mirrors
 from helpers import assert_bit_equal, small_config
 from test_cpu_denoise import random_film
 from test_cpu_trap import ALBEDO_HI, ALBEDO_LO, TRAP_HI, TRAP_LO, with_fractal_albedo
@@ -33,7 +32,7 @@ def trap_config(n, res, samples, mb=1):
 
 
 def mirror_albedo(c, inp, tile=(16, 16)):
-    return ao.render_albedo(c["world"], c["camera"], inp, tile, c["integrator"], TR)
+    return mirrors.render_albedo(c["world"], c["camera"], inp, tile, c["integrator"], TR)
 
 
 @pytest.mark.parametrize("n", [1, 3, 4])
@@ -82,7 +81,7 @@ def test_trap_changes_only_fractal_hits():
 # ---- the albedo-guided filter ---------------------------------------------------------------------------------------
 def guided(planes, desc, albedo, sigma):
     h, w = planes["normal"].shape[:2]
-    rc, out = ao.denoise(w, h, planes, desc, albedo, sigma)
+    rc, out = mirrors.denoise(w, h, planes, desc, albedo, sigma)
     assert rc == L.RAYN_OK
     return {k: v.reshape(h, w, 3) for k, v in out.items()}
 
@@ -94,7 +93,7 @@ def test_infinite_sigma_equals_unguided_mirror(w, h):
     alb[0, 0, 0] = np.nan  # not even a non-finite albedo matters: the term is not added
     for it in (1, 3, 5):
         d = denoise_desc(it, 0.5, 0.3, 0.4)
-        rc, ref = dor.denoise(w, h, p, d)
+        rc, ref = mirrors.denoise(w, h, p, d)
         assert rc == L.RAYN_OK
         got = guided(p, d, alb, np.inf)
         for k in COLOR_CH:
@@ -128,7 +127,7 @@ def test_non_finite_albedo_taps():
     alb = np.full((h, w, 3), 0.5, np.float32)
     d = denoise_desc(1, 0.7, 0.5, 0.5)
     base = guided(p, d, alb, 0.2)
-    ref = dor.denoise(w, h, p, d)[1]
+    ref = mirrors.denoise(w, h, p, d)[1]
     for k in COLOR_CH:  # equal albedo everywhere: the term is 0, the unguided result
         assert_bit_equal(base[k].reshape(-1), ref[k], f"equal albedo {k}")
     alb[4, 4, 1] = np.nan
@@ -146,5 +145,5 @@ def test_argument_errors():
     p = random_film(4, 4, 1)
     alb = np.zeros((4, 4, 3), np.float32)
     for sigma in (0.0, -1.0, np.nan, 1e-30):
-        rc, _ = ao.denoise(4, 4, p, denoise_desc(2, 0.5, 0.5, 0.5), alb, sigma)
+        rc, _ = mirrors.denoise(4, 4, p, denoise_desc(2, 0.5, 0.5, 0.5), alb, sigma)
         assert rc == L.RAYN_ERR_INVALID_ARG, sigma

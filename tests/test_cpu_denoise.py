@@ -1,4 +1,4 @@
-"""The film denoiser's CPU mirror (tests/denoise_oracle.cpp) against the properties of the a-trous statement and an
+"""The film denoiser's CPU mirror (tests/film_mirror.cpp) against the properties of the a-trous statement and an
 independent float64 numpy restatement; the ABI struct layout; Film.denoise's argument check.  No GPU needed."""
 import ctypes as C
 import os
@@ -10,7 +10,7 @@ import pytest
 from rayn_b200 import _lib as L
 from rayn_b200.film import Film, denoise_desc
 
-import denoise_oracle as dor
+import mirrors
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H5 = np.array([0.0625, 0.25, 0.375, 0.25, 0.0625])
@@ -26,7 +26,7 @@ def random_film(w, h, seed):
 
 def mirror(planes, desc):
     h, w = planes["normal"].shape[:2]
-    rc, out = dor.denoise(w, h, planes, desc)
+    rc, out = mirrors.denoise(w, h, planes, desc)
     assert rc == L.RAYN_OK
     return {k: v.reshape(h, w, 3) for k, v in out.items()}
 
@@ -57,8 +57,8 @@ def numpy_f64(planes, key, iterations, sc, sn, sa):
 
 def test_exp_of_minus_zero_is_exactly_one():
     """The centre tap has e = 0; dm::exp(-0.0f) must be exactly 1.0f, so the centre weight is h*h and sum w > 0."""
-    assert dor.exp(np.float32(-0.0)).view(np.uint32) == np.float32(1.0).view(np.uint32)
-    assert dor.exp(np.float32(0.0)).view(np.uint32) == np.float32(1.0).view(np.uint32)
+    assert mirrors.exp(np.float32(-0.0)).view(np.uint32) == np.float32(1.0).view(np.uint32)
+    assert mirrors.exp(np.float32(0.0)).view(np.uint32) == np.float32(1.0).view(np.uint32)
 
 
 def test_constant_image_stays_constant():
@@ -137,7 +137,7 @@ def test_infinite_sigmas_give_the_plain_a_trous_smoothing():
 def test_mirror_rejects_bad_descriptors(field, value):
     d = denoise_desc(3, 0.5, 0.5, 0.5)
     setattr(d, field, value)
-    rc, _ = dor.denoise(4, 4, random_film(4, 4, 7), d)
+    rc, _ = mirrors.denoise(4, 4, random_film(4, 4, 7), d)
     assert rc == L.RAYN_ERR_INVALID_ARG
 
 

@@ -49,17 +49,16 @@ def test_oracle_renders_limit_scenes(oracle, shape, volume):
 
 @pytest.mark.parametrize("shape", ["A", "B"])
 def test_trap_oracles_render_every_trap_material(shape):
-    import albedo_oracle
-    import trap_oracle
+    import mirrors
     cam, world = S.SHAPES[shape]((32, 24), True, traps=True)
     traps = world.albedo_traps()
     assert [t.material for t in traps] == S.TRAPPABLE and traps[-1].material == S.N - 1
     integ, inp = S.inputs((32, 24), 1, 3)
-    o, _ = trap_oracle.render(world, cam, inp, (8, 8), integ, S.TR)
+    o, _ = mirrors.render(world, cam, inp, (8, 8), integ, S.TR)
     _assert_sane(o, f"trap shape {shape}")
-    plain, _ = trap_oracle.render(world, cam, inp, (8, 8), integ, S.TR, traps=[])
+    plain, _ = mirrors.render(world, cam, inp, (8, 8), integ, S.TR, traps=[])
     assert not np.array_equal(o["color"], plain["color"])  # the traps show
-    alb, _ = albedo_oracle.render_albedo(world, cam, inp, (8, 8), integ, S.TR)
+    alb, _ = mirrors.render_albedo(world, cam, inp, (8, 8), integ, S.TR)
     assert np.isfinite(alb).all() and alb.max() > 0
 
 

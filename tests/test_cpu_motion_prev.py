@@ -1,4 +1,4 @@
-"""CPU mirror of the motion plane against an explicit previous scene (rayn_b200_render_motion_prev, tests/motion_prev_oracle.cpp)
+"""CPU mirror of the motion plane against an explicit previous scene (rayn_b200_render_motion_prev, tests/render_mirror.cpp)
 against float64 closed forms: a pinhole camera orbiting a static scene, a cut to an unrelated pose, a zoom, an orthographic pan,
 a thin-lens camera, a static sphere displaced between frames and a moving sphere whose velocity changes.  Also the header's
 identity with render_motion when prev is the uploaded scene, the argument rules of the mirror, the chord of closure parameters
@@ -12,8 +12,7 @@ from rayn_b200 import _lib as L
 from rayn_b200 import configs
 from rayn_b200.scene import Linear, OrthographicCamera, PinholeCamera, Sphere, ThinLensCamera, Vec3
 
-import motion_prev_oracle as mpo
-import temporal_oracle as to
+import mirrors
 from helpers import assert_bit_equal, small_config
 from test_cpu_temporal import ORIGIN, basis, proj64
 
@@ -61,7 +60,7 @@ def check(per, geo, cur, prev, moved_fn=None, min_valid=0.5, min_motion=0.05):
 
 def prev_motion(c, cam, prev_cam, prev_world=None, inp=None):
     d, p, keep = descs(c["world"], cam, prev_cam, prev_world)
-    _, per, geo = mpo.render_motion_prev(d, p, inp, (8, 8), c["integrator"], TR, DT, geometry=True)
+    _, per, geo = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=p, geometry=True)
     return per, geo, d.camera, p.camera
 
 
@@ -139,7 +138,7 @@ def test_static_sphere_displaced():
     sphere_world(prev_world, Vec3(*c0), 0.3)
     d, p, keep = descs(c["world"], c["camera"], prev_world["camera"], prev_world["world"])
     assert p.hitables[j].center[0] != d.hitables[j].center[0]
-    _, per, geo = mpo.render_motion_prev(d, p, inp, (8, 8), c["integrator"], TR, DT, geometry=True)
+    _, per, geo = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=p, geometry=True)
     c1f, c0f = np.array(d.hitables[j].center[:], np.float64), np.array(p.hitables[j].center[:], np.float64)
 
     def moved(P, tau):
@@ -163,7 +162,7 @@ def test_moving_sphere_changes_velocity():
     prev_world, _ = small_config(3, (W, H), 2, 1)
     sphere_world(prev_world, Linear(Vec3(*(base - 0.1 * bu)), Vec3(*v0)), 0.3)
     d, p, keep = descs(c["world"], c["camera"], prev_world["camera"], prev_world["world"])
-    _, per, geo = mpo.render_motion_prev(d, p, inp, (8, 8), c["integrator"], TR, DT, geometry=True)
+    _, per, geo = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=p, geometry=True)
     h, hp = d.hitables[j], p.hitables[j]
     ctr = lambda hh, t: np.array(hh.center[:], np.float64) + np.array(hh.center_velocity[:], np.float64) * t[:, None]  # noqa: E731
 
@@ -184,8 +183,8 @@ def test_prev_equal_to_the_uploaded_scene_is_render_motion(n):
     cams = [c["camera"]] + ([moving_cameras(c, (29, 21))[k] for k in ("pan", "dolly", "ortho", "thinlens")] if n == 3 else [])
     for cam in cams:
         d, keep = c["world"].flatten(cam)
-        a = to.render_motion(c["world"], cam, inp, (8, 8), c["integrator"], TR, DT)
-        b = mpo.render_motion_prev(d, d, inp, (8, 8), c["integrator"], TR, DT)
+        a = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT)
+        b = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=d)
         assert_bit_equal(b[0], a[0], f"cfg{n} plane")
         assert_bit_equal(b[1], a[1], f"cfg{n} records")
 
@@ -194,8 +193,8 @@ def test_moving_sphere_differs_from_render_motion_by_rounding_only():
     c, inp = small_config(3, (29, 21), 2, 1)
     sphere_world(c, Linear(Vec3(-1.0, 0.4, 0.9), Vec3(4.0, 0.0, 1.0)), 0.35)
     d, keep = c["world"].flatten(c["camera"])
-    _, a = to.render_motion(c["world"], c["camera"], inp, (8, 8), c["integrator"], TR, DT)
-    _, b = mpo.render_motion_prev(d, d, inp, (8, 8), c["integrator"], TR, DT)
+    _, a = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT)
+    _, b = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=d)
     ok = ~np.isnan(a[..., 2])
     assert_bit_equal(np.isnan(b[..., 2]), ~ok)
     assert (a[..., 0][ok] != 0).any()
@@ -213,7 +212,8 @@ def changed_kind(d):
 
 
 def test_mirror_argument_rules():
-    """NULL prev, another camera kind, another hitable count or another hitable kind: RAYN_ERR_INVALID_ARG"""
+    """a previous scene without hitables, another camera kind, another hitable count or another hitable kind:
+    RAYN_ERR_INVALID_ARG (a NULL prev is the uploaded scene run backwards, render_motion's statement)"""
     c, inp = small_config(3, (8, 8), 1, 1)
     d, k = c["world"].flatten(c["camera"])
     ortho = c["world"].cameras.add_camera(OrthographicCamera((8, 8), 2.0, Vec3(9.5, -3.5, 9.5), Vec3(0, 0, 0), Vec3(0, 1, 0)))
@@ -222,9 +222,11 @@ def test_mirror_argument_rules():
     sphere_world(c2, Vec3(0, 0, 0), 0.1)
     p_n, kn = c2["world"].flatten(c2["camera"])
     p_kind, kk = changed_kind(d)
-    for bad in (None, p_cam, p_n, p_kind):
+    p_none = L.RaynSceneDesc.from_buffer_copy(d)
+    p_none.hitables = None
+    for bad in (p_none, p_cam, p_n, p_kind):
         with pytest.raises(RuntimeError) as e:
-            mpo.render_motion_prev(d, bad, inp, (8, 8), c["integrator"], TR, DT)
+            mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=bad)
         assert e.value.args[0] == L.RAYN_ERR_INVALID_ARG
 
 

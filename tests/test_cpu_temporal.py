@@ -1,5 +1,5 @@
-"""CPU mirrors of the motion plane (tests/motion_oracle.cpp), the temporal push and the scaled variance denoise
-(tests/temporal_oracle.cpp): the motion records against float64 closed forms (a pinhole camera translating sideways past the
+"""CPU mirrors of the motion plane (tests/render_mirror.cpp), the temporal push and the scaled variance denoise
+(tests/film_mirror.cpp): the motion records against float64 closed forms (a pinhole camera translating sideways past the
 scene, a sphere moving in front of a static camera), the identities the header guarantees (static scenes give dx = dy = +0 and
 z_prev == z; alpha = 1 returns the frame bit for bit with s = 1; a cumulative mean gives s = 1/n; a unit scale is the unscaled
 filter), the argument rules and the RaynTemporalDesc layout."""
@@ -15,8 +15,7 @@ from rayn_b200 import configs
 from rayn_b200.film import denoise_desc
 from rayn_b200.scene import Lambertian, Linear, PinholeCamera, Sphere, Vec3
 
-import moments_oracle as mo
-import temporal_oracle as to
+import mirrors
 from helpers import assert_bit_equal, small_config
 from test_cpu_denoise import random_film
 
@@ -44,7 +43,7 @@ def add_camera(c, cam):
 def test_static_scene_gives_exact_zero_motion():
     """a static camera and scene: both projections are the same function of the same point, so dx = dy = +0 and z_prev == z"""
     c, inp = small_config(3, (23, 17), 2, 1)
-    plane, per = to.render_motion(c["world"], c["camera"], inp, (8, 8), c["integrator"], TR, DT)
+    plane, per = mirrors.render_motion(c["world"].flatten(c["camera"])[0], inp, (8, 8), c["integrator"], TR, DT)
     valid = ~np.isnan(per[..., 2])
     assert valid.any()
     assert (per[..., :2][valid].view(np.uint32) == 0).all()
@@ -63,7 +62,7 @@ def test_camera_translating_sideways():
     vel = Vec3(*(v * bu))
     cam = add_camera(c, PinholeCamera((W, H), 60.0, Linear(Vec3(*ORIGIN), vel), Linear(Vec3(0, 0, 0), vel), Vec3(0, 1, 0)))
     hx = camera_desc(c["world"], cam).half_size[0]
-    _, per = to.render_motion(c["world"], cam, inp, (8, 8), c["integrator"], TR, DT)
+    _, per = mirrors.render_motion(c["world"].flatten(cam)[0], inp, (8, 8), c["integrator"], TR, DT)
     valid = ~np.isnan(per[..., 2])
     assert valid.mean() > 0.9
     z = per[..., 2][valid].astype(np.float64)
@@ -83,7 +82,7 @@ def test_sphere_moving_in_front_of_a_static_camera():
     mat = c["world"].materials.add_material(Lambertian((0.5, 0.5, 0.5)))
     c["world"].hitables.push(Sphere(Linear(Vec3(*centre), Vec3(*(s * bu))), 0.3, mat))
     hx = camera_desc(c["world"], c["camera"]).half_size[0]
-    _, per = to.render_motion(c["world"], c["camera"], inp, (8, 8), c["integrator"], TR, DT)
+    _, per = mirrors.render_motion(c["world"].flatten(c["camera"])[0], inp, (8, 8), c["integrator"], TR, DT)
     valid = ~np.isnan(per[..., 2])
     moving = valid & (per[..., 0] != 0)
     assert 0.02 < moving.mean() < 0.9
@@ -97,7 +96,7 @@ def test_resolve_is_the_mean_over_valid_samples():
     c, inp = small_config(3, (21, 13), 2, 1)
     bu, _ = basis(ORIGIN, np.zeros(3))
     cam = add_camera(c, PinholeCamera((21, 13), 60.0, Linear(Vec3(*ORIGIN), Vec3(*(0.5 * bu))), Vec3(0, 0, 0), Vec3(0, 1, 0)))
-    plane, per = to.render_motion(c["world"], cam, inp, (8, 8), c["integrator"], TR, DT)
+    plane, per = mirrors.render_motion(c["world"].flatten(cam)[0], inp, (8, 8), c["integrator"], TR, DT)
     ok = ~np.isnan(per[..., 2])
     n = ok.sum(axis=2)
     s = np.where(ok[..., None], per, 0).astype(np.float64).sum(axis=2)
@@ -109,7 +108,7 @@ def test_resolve_is_the_mean_over_valid_samples():
 def test_tile_grid_quirk_pixels_never_match():
     """film.rs:399-404: a 20-wide film with 16-wide tiles has one tile column; pixels 16..19 get (0, 0, +inf, +inf)"""
     c, inp = small_config(3, (20, 9), 1, 1)
-    plane, _ = to.render_motion(c["world"], c["camera"], inp, (16, 16), c["integrator"], TR, DT)
+    plane, _ = mirrors.render_motion(c["world"].flatten(c["camera"])[0], inp, (16, 16), c["integrator"], TR, DT)
     assert (plane[:, 16:, :2] == 0).all() and np.isposinf(plane[:, 16:, 2:]).all()
     assert np.isfinite(plane[:, :16, 2]).any()
 
@@ -132,7 +131,7 @@ def frame(w, h, seed, static=True):
 
 def test_alpha_one_returns_every_frame_unchanged():
     w, h = 17, 11
-    t = to.TemporalMirror(w, h)
+    t = mirrors.TemporalMirror(w, h)
     for k in range(4):
         p, m, mv = frame(w, h, 40 + k, static=False)
         rc, out, om, s = t.push(p, m, mv, 1.0, 0.1, -1.0)
@@ -145,7 +144,7 @@ def test_alpha_one_returns_every_frame_unchanged():
 def test_cumulative_mean_on_a_static_view():
     """alpha_min -> 0, no motion, equal depths and normals: the blend is the running mean, s = 1/n"""
     w, h = 13, 9
-    t = to.TemporalMirror(w, h)
+    t = mirrors.TemporalMirror(w, h)
     frames = [frame(w, h, 60 + k) for k in range(6)]
     for k, (p, m, mv) in enumerate(frames):
         p["normal"] = frames[0][0]["normal"]
@@ -159,7 +158,7 @@ def test_cumulative_mean_on_a_static_view():
 
 def test_reset_and_disocclusion_take_the_current_frame():
     w, h = 15, 10
-    t = to.TemporalMirror(w, h)
+    t = mirrors.TemporalMirror(w, h)
     p0, m0, mv0 = frame(w, h, 80)
     t.push(p0, m0, mv0, 0.2, 0.05, 0.5)
     p1, m1, mv1 = frame(w, h, 81)
@@ -178,14 +177,14 @@ def test_reset_and_disocclusion_take_the_current_frame():
 @pytest.mark.parametrize("field,value", [("alpha_min", 0.0), ("alpha_min", 1.5), ("alpha_min", np.nan), ("sigma_depth", 0.0),
                                          ("normal_cos", 1.5), ("normal_cos", np.nan), ("reset", 2)])
 def test_mirror_rejects_bad_descriptors(field, value):
-    t = to.TemporalMirror(4, 4)
+    t = mirrors.TemporalMirror(4, 4)
     p, m, mv = frame(4, 4, 1)
     kw = dict(alpha_min=0.2, sigma_depth=0.1, normal_cos=0.5, reset=False)
     kw[field] = value
     if field == "reset":
         d = L.RaynTemporalDesc(0.2, 0.1, 0.5, value)
         z = np.zeros(16 * 14, np.float32)
-        rc = to.temporal_lib().rayn_oracle_temporal_push(4, 4, C.byref(d), *([z.ctypes.data] * 13))
+        rc = mirrors.film_lib().rayn_oracle_temporal_push(4, 4, C.byref(d), *([z.ctypes.data] * 13))
     else:
         rc = t.push(p, m, mv, **kw)[0]
     assert rc == L.RAYN_ERR_INVALID_ARG
@@ -196,12 +195,12 @@ def test_unit_scale_is_the_unscaled_filter():
     p = random_film(w, h, 90)
     m = np.random.default_rng(90).uniform(0, 2, (h, w, 2)).astype(np.float32)
     d = denoise_desc(3, np.inf, 0.5, 0.5)
-    rc0, a = mo.denoise(w, h, p, d, 4.0, 16, m)
-    rc1, b = to.denoise_scaled(w, h, p, d, 4.0, 16, m, np.ones((h, w), np.float32))
+    rc0, a = mirrors.denoise(w, h, p, d, moments=m, spp=16, sigma_luminance=4.0)
+    rc1, b = mirrors.denoise(w, h, p, d, moments=m, spp=16, sigma_luminance=4.0, var_scale=np.ones((h, w), np.float32))
     assert rc0 == rc1 == 0
     for k in a:
         assert_bit_equal(b[k], a[k], k)
-    rc2, c_ = to.denoise_scaled(w, h, p, d, 4.0, 16, m, np.full((h, w), 0.25, np.float32))
+    rc2, c_ = mirrors.denoise(w, h, p, d, moments=m, spp=16, sigma_luminance=4.0, var_scale=np.full((h, w), 0.25, np.float32))
     assert rc2 == 0 and not np.array_equal(c_["color"], a["color"])
 
 
@@ -220,7 +219,7 @@ def test_temporal_desc_layout_matches_the_c_compiler(tmp_path):
 def test_pixel_without_a_hit_takes_no_history():
     """a sky / miss pixel (motion (0, 0, +inf, +inf), normal 0) never matches a history tap, whatever normal_cos"""
     w, h = 9, 7
-    t = to.TemporalMirror(w, h)
+    t = mirrors.TemporalMirror(w, h)
     p0, m0, mv0 = frame(w, h, 120)
     p0["color"][:] = 1.0
     t.push(p0, m0, mv0, 0.5, 0.1, -1.0)
@@ -237,7 +236,7 @@ def test_pixel_without_a_hit_takes_no_history():
 def test_orthographic_depths_below_zero_still_match():
     """an orthographic view depth may be <= 0: the depth test compares against |z_prev|"""
     w, h = 9, 7
-    t = to.TemporalMirror(w, h)
+    t = mirrors.TemporalMirror(w, h)
     for k in range(3):
         p, m, mv = frame(w, h, 130 + k)
         mv[..., 2:] = -3.0
@@ -297,7 +296,7 @@ def test_projection_inverts_camera_ray(kind):
     W, H = 36, 26
     c, inp = small_config(3, (W, H), 2, 1)
     cam = moving_cameras(c, (W, H))[kind]
-    _, per, geo = to.render_motion(c["world"], cam, inp, (8, 8), c["integrator"], TR, DT, geometry=True)
+    _, per, geo = mirrors.render_motion(c["world"].flatten(cam)[0], inp, (8, 8), c["integrator"], TR, DT, geometry=True)
     ok = ~np.isnan(per[..., 2])
     assert ok.mean() > 0.5
     px, py, z = proj64(camera_desc(c["world"], cam), geo[..., :3][ok], geo[..., 3][ok], W, H)
@@ -312,7 +311,7 @@ def test_motion_matches_float64_projection(kind):
     W, H = 36, 26
     c, inp = small_config(3, (W, H), 2, 1)
     cam = moving_cameras(c, (W, H))[kind]
-    _, per, geo = to.render_motion(c["world"], cam, inp, (8, 8), c["integrator"], TR, DT, geometry=True)
+    _, per, geo = mirrors.render_motion(c["world"].flatten(cam)[0], inp, (8, 8), c["integrator"], TR, DT, geometry=True)
     ok = ~np.isnan(per[..., 2])
     X, t = geo[..., :3][ok], geo[..., 3][ok].astype(np.float64)
     cd = camera_desc(c["world"], cam)

@@ -1,5 +1,5 @@
 """The temporal push (rayn_b200_temporal_push) restated from the header in numpy, against the CPU mirror
-(tests/temporal_oracle.cpp, TemporalMirror) bit for bit, and against a float64 statement of its intent: bilinear history at
+(tests/film_mirror.cpp, TemporalMirror) bit for bit, and against a float64 statement of its intent: bilinear history at
 (x + dx, y + dy) in exact arithmetic.
 
 The numpy statement is written from include/rayn_b200.h, not from the mirror: taps j outer and i inner, every product and sum
@@ -21,7 +21,7 @@ import pytest
 
 from rayn_b200 import _lib as L
 
-import temporal_oracle as to
+import mirrors
 from helpers import assert_bit_equal
 
 f32 = np.float32
@@ -195,7 +195,7 @@ def mirror_push(t, cur, nrm, motion, desc, reset, alias):
     s = np.empty(npx, f32)
     d = L.RaynTemporalDesc(*(float(v) for v in desc), 1 if reset else 0)
     hin, hout = t.hist[t.cur], t.hist[t.cur ^ 1]
-    rc = to.temporal_lib().rayn_oracle_temporal_push(W, H, C.byref(d), hin.ctypes.data, hout.ctypes.data, c.ctypes.data, b.ctypes.data,
+    rc = mirrors.film_lib().rayn_oracle_temporal_push(W, H, C.byref(d), hin.ctypes.data, hout.ctypes.data, c.ctypes.data, b.ctypes.data,
                                                      n.ctypes.data, mc.ctypes.data, mb.ctypes.data, mv.ctypes.data, c.ctypes.data,
                                                      b.ctypes.data, mc.ctypes.data, mb.ctypes.data, s.ctypes.data)
     if rc == L.RAYN_OK:
@@ -208,7 +208,7 @@ def test_numpy_statement_equals_the_mirror(W, H):
     """16 pushes with edge-case motion, spoiled histories, every descriptor of DESCS, random resets and aliased outputs: the
     numpy statement and the mirror agree on every output and on the history they write, bit for bit"""
     rng = np.random.default_rng(1000 * W + H)
-    t = to.TemporalMirror(W, H)
+    t = mirrors.TemporalMirror(W, H)
     npx = W * H
     for k in range(2 * len(DESCS)):
         cur, nrm, motion = edge_frame(W, H, rng)
@@ -232,7 +232,7 @@ def test_the_edge_inputs_reach_every_rule():
     exactly 1 and 0, the copy path and the blend"""
     W, H = 31, 31
     rng = np.random.default_rng(5)
-    t = to.TemporalMirror(W, H)
+    t = mirrors.TemporalMirror(W, H)
     counts = {}
     # 16 pushes: every descriptor of DESCS twice
     seen = dict(copy=0, blend=0, n_frac=0, half=0, nonfinite=0, weight_rounds_to_zero=0)
@@ -264,7 +264,7 @@ def test_float64_intent_on_well_conditioned_inputs():
     is the float64 bilinear reprojection at (x + dx, y + dy) within 1e-5 relative, over 8 pushes"""
     W, H = 41, 29
     rng = np.random.default_rng(11)
-    t = to.TemporalMirror(W, H)
+    t = mirrors.TemporalMirror(W, H)
     npx = W * H
     nrm = np.tile(np.array([[0.0], [0.6], [0.8]], f32), npx)
     for k in range(8):
@@ -319,7 +319,7 @@ def test_mirror_rejects_films_wider_or_taller_than_two_to_the_23():
     d = L.RaynTemporalDesc(0.2, 0.1, 0.5, 0)
     z = np.zeros(14, np.float32)
     for W, H in ((MAX_SIDE + 1, 1), (1, MAX_SIDE + 1)):
-        rc = to.temporal_lib().rayn_oracle_temporal_push(W, H, C.byref(d), *([z.ctypes.data] * 13))
+        rc = mirrors.film_lib().rayn_oracle_temporal_push(W, H, C.byref(d), *([z.ctypes.data] * 13))
         assert rc == L.RAYN_ERR_INVALID_ARG, (W, H)
 
 
@@ -344,7 +344,7 @@ def variance_ratio(dx, dy, seed):
     the last frame, on the pixels whose history chain stays inside the image"""
     N = STAT_N
     rng = np.random.default_rng(seed)
-    t = to.TemporalMirror(N, N)
+    t = mirrors.TemporalMirror(N, N)
     nrm = np.zeros((N, N, 3), f32)
     nrm[..., 2] = 1.0
     mv = np.zeros((N, N, 4), f32)
@@ -401,7 +401,7 @@ def test_history_without_a_hit_is_never_used(sigma_depth):
     mirror and in the numpy statement"""
     W, H = 4, 3
     (p0, m0, mv0), (p1, m1, mv1) = sky_then_hit(W, H, np.random.default_rng(4))
-    t = to.TemporalMirror(W, H)
+    t = mirrors.TemporalMirror(W, H)
     t.push(p0, m0, mv0, 0.2, sigma_depth, -1.0)
     hin = t.hist[t.cur].copy()
     rc, out, om, s = t.push(p1, m1, mv1, 0.2, sigma_depth, -1.0)

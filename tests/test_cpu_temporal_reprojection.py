@@ -1,6 +1,6 @@
 """Reprojection of rendered frames through the temporal push, end to end on the CPU mirrors: the motion plane of frame k
-(tests/motion_oracle.cpp, tests/motion_prev_oracle.cpp) must carry frame k-1's history to where frame k sees the same
-surface point (tests/temporal_oracle.cpp).
+(tests/render_mirror.cpp) must carry frame k-1's history to where frame k sees the same
+surface point (tests/film_mirror.cpp).
 
 Config 1's world with the camera 1.35 from the centre of its unit sphere, so the sphere fills the view and depth is smooth;
 shutter 0, frames k-1 and k.  Frame k-1 is pushed into a new history with its per-pixel mean world-space hit point P as colour
@@ -37,8 +37,7 @@ from rayn_b200 import configs
 from rayn_b200.film import FrameInputs
 from rayn_b200.scene import Linear, OrthographicCamera, PinholeCamera, Sphere, Vec3
 
-import motion_prev_oracle as mpo
-import temporal_oracle as to
+import mirrors
 
 f32 = np.float32
 DT = 1.0 / 24.0
@@ -115,9 +114,9 @@ def render_pair(motion, W, H, samples, device=None):
     out = {"camera": d1.camera, "v": v}
     for i, (d, p, inp, tr) in enumerate(((d0, d0, inps[0], shutter0(K - 1)), (d1, d0, inps[1], shutter0(K)))):
         if prev:
-            plane, per, geo = mpo.render_motion_prev(d, p, inp, TILE, c["integrator"], tr, DT, geometry=True)
+            plane, per, geo = mirrors.render_motion(d, inp, TILE, c["integrator"], tr, DT, prev=p, geometry=True)
         else:
-            plane, per, geo = to.render_motion(c["world"], cam, inp, TILE, c["integrator"], tr, DT, geometry=True)
+            plane, per, geo = mirrors.render_motion(c["world"].flatten(cam)[0], inp, TILE, c["integrator"], tr, DT, geometry=True)
         if device is not None:
             out[f"mirror_plane{i}"] = plane
             device.upload_scene(c["world"], cam, tr)
@@ -177,7 +176,7 @@ def check(res, max_error):
 
 
 def mirror_push(W, H):
-    t = to.TemporalMirror(W, H)
+    t = mirrors.TemporalMirror(W, H)
 
     def push(planes, moments, motion, alpha_min, sigma_depth, normal_cos, reset):
         rc, out, om, s = t.push(planes, moments, motion, alpha_min, sigma_depth, normal_cos, reset)

@@ -1,4 +1,4 @@
-"""Orbit-trap albedo on the CPU (include/rayn_b200.h, RaynAlbedoTrap): the trap oracle's trap and palette (tests/trap_oracle.cpp)
+"""Orbit-trap albedo on the CPU (include/rayn_b200.h, RaynAlbedoTrap): the trap oracle's trap and palette (tests/render_mirror.cpp)
 against the numpy restatement in tests/trap_mirror.py bit for bit, identity films against the render oracle that pin the trap
 plumbing, and the ABI."""
 import ctypes as C
@@ -49,10 +49,10 @@ def trap_points(seed, n=4000):
 
 @pytest.fixture(scope="module")
 def toracle():
-    """the orbit-trap oracle (tests/trap_oracle.py): the render oracle of oracle/ plus trap, palette and per-lane albedo"""
-    import trap_oracle
-    trap_oracle.lib()
-    return trap_oracle
+    """the orbit-trap oracle (tests/mirrors.py): the render oracle of oracle/ plus trap, palette and per-lane albedo"""
+    import mirrors
+    mirrors.render_lib()
+    return mirrors
 
 
 def unfused_only():
@@ -121,7 +121,7 @@ def render_with(binding, c, inp):
 def test_identity_films(oracle, toracle, n, lo, hi, which):
     """s == 1 (every trap >= 0 > trap_hi) gives albedo_hi exactly, s == 0 (every finite trap < trap_lo) albedo_lo: the trap
     oracle's film equals the render oracle's constant-albedo film bit for bit, so the trap plumbing (the per-lane split of
-    integrate in tests/trap_oracle.cpp) moved no sample."""
+    integrate in tests/render_mirror.cpp) moved no sample."""
     c, inp = small_config(n, (21, 13), 1, 3)
     with_fractal_albedo(c, OrbitTrapAlbedo(lo, hi, ALBEDO_LO, ALBEDO_HI))
     assert len(c["world"].albedo_traps()) == 1

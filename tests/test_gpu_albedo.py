@@ -1,6 +1,6 @@
 """First-hit albedo plane on the device (rayn_b200_render_albedo, rt_albedo.cuh) against its CPU mirror
-(tests/albedo_oracle.cpp) bit for bit, and the albedo-guided denoise (rayn_b200_film_denoise_albedo) against its mirror
-(tests/denoise_albedo_oracle.cpp): odd sizes and tile shapes with and without traps, a trap material shared by a sphere and the
+(tests/render_mirror.cpp) bit for bit, and the albedo-guided denoise (rayn_b200_film_denoise_albedo) against its mirror
+(tests/film_mirror.cpp): odd sizes and tile shapes with and without traps, a trap material shared by a sphere and the
 Mandelbox, fold-all on and off, moving spheres, thin-lens and orthographic cameras, sampled tiles of a full-size film, host and
 device planes, the alpha identity at full size, the golden fixture, no side effects on later renders, argument errors and the
 Film / Renderer interfaces."""
@@ -15,8 +15,7 @@ from rayn_b200 import configs
 from rayn_b200.film import ALBEDO_SAMPLES, DENOISE_ALBEDO_SIGMA, Film, FrameInputs, Renderer, denoise_desc, make_frame_desc
 from rayn_b200.scene import Lambertian, Sphere, Vec3
 
-import albedo_oracle as ao
-import denoise_oracle as dor
+import mirrors
 from helpers import CH, assert_bit_equal, small_config
 from test_cpu_albedo import trap_config, white
 from test_cpu_denoise import random_film
@@ -34,7 +33,7 @@ def gpu_albedo(r, c, inp, tile, camera=None):
 
 
 def mirror(c, inp, tile, camera=None):
-    return ao.render_albedo(c["world"], camera if camera is not None else c["camera"], inp, tile, c["integrator"], TR)[0]
+    return mirrors.render_albedo(c["world"], camera if camera is not None else c["camera"], inp, tile, c["integrator"], TR)[0]
 
 
 @pytest.mark.parametrize("n", [1, 2, 3, 4, 5])
@@ -79,7 +78,7 @@ def test_full_size_cfg3_trap_sampled_tiles(renderer):
     c, _ = trap_config(3, (1920, 1080), 1)
     inp = FrameInputs(1920, 1080, 1, c["integrator"])
     g = gpu_albedo(renderer, c, inp, (16, 16))
-    o = ao.render_albedo(c["world"], c["camera"], inp, (16, 16), c["integrator"], TR, subsample_k=97)[0]  # every 97th tile
+    o = mirrors.render_albedo(c["world"], c["camera"], inp, (16, 16), c["integrator"], TR, subsample_k=97)[0]  # every 97th tile
     nty = (1080 + 1080 % 16) // 16
     for t in range(0, 120 * nty, 97):
         tx, ty = t // nty, t % nty
@@ -214,7 +213,7 @@ def gpu_guided(r, planes, desc, albedo, sigma, w, h):
 
 def check_guided(r, planes, desc, albedo, sigma, w, h, what):
     g = gpu_guided(r, planes, desc, albedo, sigma, w, h)
-    rc, o = ao.denoise(w, h, planes, desc, albedo, sigma)
+    rc, o = mirrors.denoise(w, h, planes, desc, albedo, sigma)
     assert rc == L.RAYN_OK and set(g) == set(o)
     for k in g:
         assert_bit_equal(g[k], o[k], f"{what} {k}")
@@ -240,7 +239,7 @@ def test_guided_absent_planes_spaces_and_aliasing(renderer):
     d = denoise_desc(5, 0.5, 0.3, 0.3)
     check_guided(renderer, {k: v for k, v in p.items() if k != "background"}, d, alb, 0.1, w, h, "NULL background")
     check_guided(renderer, {k: v for k, v in p.items() if k != "color"}, d, alb, 0.1, w, h, "NULL color")
-    rc, ref = ao.denoise(w, h, p, d, alb, 0.1)
+    rc, ref = mirrors.denoise(w, h, p, d, alb, 0.1)
     assert rc == L.RAYN_OK
     flat = {k: np.ascontiguousarray(v).reshape(-1) for k, v in p.items()}
     flat["albedo"] = alb.reshape(-1)
@@ -329,7 +328,7 @@ def test_film_albedo_channel(tmp_path):
         for k in COLOR_CH:
             assert_bit_equal(film.channels[k], plain.channels[k], f"Film.denoise at the default sigma {k}")
     else:
-        rc, ref = ao.denoise(48, 32, {**before, "normal": film.channels["normal"], "alpha": film.channels["alpha"]}, denoise_desc(3),
+        rc, ref = mirrors.denoise(48, 32, {**before, "normal": film.channels["normal"], "alpha": film.channels["alpha"]}, denoise_desc(3),
                              film.channels["albedo"], DENOISE_ALBEDO_SIGMA)
         for k in COLOR_CH:
             assert_bit_equal(film.channels[k].reshape(-1), ref[k], f"Film.denoise {k}")

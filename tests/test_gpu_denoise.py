@@ -1,4 +1,4 @@
-"""GPU film denoiser (rayn_b200_film_denoise, rt_denoise.cuh) against its CPU mirror (tests/denoise_oracle.cpp), bit for
+"""GPU film denoiser (rayn_b200_film_denoise, rt_denoise.cuh) against its CPU mirror (tests/film_mirror.cpp), bit for
 bit: random planes, rendered films, every level count, host and device spaces, aliasing, absent planes; argument
 errors; the exact zero-weight cutoff of dm::exp on the device; image quality; and that rendering is unaffected."""
 import ctypes as C
@@ -13,7 +13,7 @@ from rayn_b200 import _lib as L
 from rayn_b200 import configs
 from rayn_b200.film import Film, denoise_desc
 
-import denoise_oracle as dor
+import mirrors
 from helpers import CH, assert_bit_equal, small_config
 from test_cpu_denoise import random_film
 
@@ -42,7 +42,7 @@ def _call(renderer, planes, desc, w, h):
 
 def check_against_mirror(renderer, planes, desc, w, h, what):
     g = gpu(renderer, planes, desc, w, h)
-    rc, o = dor.denoise(w, h, planes, desc)
+    rc, o = mirrors.denoise(w, h, planes, desc)
     assert rc == L.RAYN_OK
     assert set(g) == set(o)
     for k in g:
@@ -86,7 +86,7 @@ def test_device_spaces_and_aliasing(renderer):
     w, h = 67, 45
     p = random_film(w, h, 10)
     d = denoise_desc(5, 0.5, 0.3, 0.3)
-    rc, ref = dor.denoise(w, h, p, d)
+    rc, ref = mirrors.denoise(w, h, p, d)
     assert rc == L.RAYN_OK
     flat = {k: np.ascontiguousarray(v).reshape(-1) for k, v in p.items()}
     lib = L.lib()
@@ -137,7 +137,7 @@ def test_film_denoise_in_place(renderer):
     f.render_frame_into(c["world"], c["camera"], c["integrator"], None, (16, 16), 1, TR, c["samples"])
     before = {k: v.copy() for k, v in f.channels.items()}
     f.denoise(3, sigma_color=0.4)
-    rc, o = dor.denoise(40, 32, before, denoise_desc(3, 0.4))
+    rc, o = mirrors.denoise(40, 32, before, denoise_desc(3, 0.4))
     for k in COLOR_CH:
         assert f.channels[k].shape == (32, 40, 3)
         assert_bit_equal(f.channels[k].reshape(-1), o[k], f"Film.denoise {k}")
@@ -220,7 +220,7 @@ def test_cpp_host_denoise_flag(tmp_path):
         raw = np.fromfile(path, np.float32)
         return {"color": raw[:3 * npx], "alpha": raw[3 * npx:4 * npx], "background": raw[4 * npx:7 * npx], "normal": raw[7 * npx:]}
     raw, den = planes(tmp_path / "raw.bin"), planes(tmp_path / "den.bin")
-    rc, o = dor.denoise(48, 32, raw, denoise_desc(4))
+    rc, o = mirrors.denoise(48, 32, raw, denoise_desc(4))
     assert rc == L.RAYN_OK
     for k in COLOR_CH:
         assert_bit_equal(den[k], o[k], f"rayn_host --denoise {k}")

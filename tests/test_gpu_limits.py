@@ -13,9 +13,8 @@ from rayn_b200 import _lib as L
 from rayn_b200 import Emissive, Srgb
 from rayn_b200.film import Renderer, tile_grid
 
-import albedo_oracle
 import limits_scenes as S
-import trap_oracle
+import mirrors
 from helpers import CH, assert_bit_equal, random_rays, small_config
 from test_cpu_limits import FAMILIES, K_FRAMES, check_sphere_closest_hit, closed_form_films, sphere_rays
 
@@ -36,7 +35,7 @@ def gpu_render(r, world, cam, inp, integ, tile, **kw):
 def oracle_render(oracle, world, cam, inp, integ, tile, **kw):
     """the trap oracle for worlds with orbit-trap albedos, the plain oracle otherwise"""
     if world.albedo_traps():
-        return trap_oracle.render(world, cam, inp, tile, integ, TR, **kw)
+        return mirrors.render(world, cam, inp, tile, integ, TR, **kw)
     return oracle.render(world, cam, inp, tile, integ, TR, **kw)
 
 
@@ -174,7 +173,7 @@ def test_orbit_traps_on_every_trappable_material(renderer, oracle, shape):
     def albedo(r):
         r.upload_scene(world, cam)
         return r.render_albedo(inp, tile, integ, TR)
-    want = albedo_oracle.render_albedo(world, cam, inp, tile, integ, TR)[0]
+    want = mirrors.render_albedo(world, cam, inp, tile, integ, TR)[0]
     for flags in (0, L.FLAG_NO_FOLD_ALL):
         assert_bit_equal(with_renderer(albedo, flags=flags), want, f"albedo {shape} flags {flags}")
 

@@ -1,6 +1,6 @@
 """Luminance moments on the device (rayn_b200_render_frame_moments, k_resolve<true>) against their CPU mirror
-(tests/moments_oracle.cpp) bit for bit, and the variance-guided denoise (rayn_b200_film_denoise_variance) against its mirror
-(tests/denoise_variance_oracle.cpp): configs 1-5 at odd sizes and two tile shapes, traps, fold-all on and off, moving spheres and
+(tests/render_mirror.cpp) bit for bit, and the variance-guided denoise (rayn_b200_film_denoise_variance) against its mirror
+(tests/film_mirror.cpp): configs 1-5 at odd sizes and two tile shapes, traps, fold-all on and off, moving spheres and
 the thin-lens / orthographic cameras, several passes, sampled tiles of a full-size film, host and device planes, NULL planes,
 film planes equal to render_frame's, render_frame and render_frame_moments alternated through the graph cache, the golden
 fixture, argument errors and the Film / Renderer interfaces."""
@@ -15,7 +15,7 @@ from rayn_b200 import configs
 from rayn_b200.film import Film, FrameInputs, Renderer, denoise_desc, make_frame_desc
 from rayn_b200.scene import Lambertian, Sphere, Vec3
 
-import moments_oracle as mo
+import mirrors
 from helpers import CH, assert_bit_equal, small_config
 from test_cpu_albedo import trap_config
 from test_cpu_moments import moment_film
@@ -33,7 +33,7 @@ def gpu(r, c, inp, tile, camera=None):
 
 
 def mirror(c, inp, tile, camera=None, **kw):
-    return mo.render(c["world"], camera if camera is not None else c["camera"], inp, tile, c["integrator"], TR, **kw)
+    return mirrors.render(c["world"], camera if camera is not None else c["camera"], inp, tile, c["integrator"], TR, moments=True, **kw)[0]
 
 
 def check(g, o, what):
@@ -282,7 +282,7 @@ def test_simple_march_is_unsupported_inner():
 def check_var(r, planes, desc, sl, spp, m, w, h, what, albedo=None, sa=np.inf):
     g = r.denoise(w, h, planes, desc.iterations, desc.sigma_color, desc.sigma_normal, desc.sigma_alpha, albedo=albedo,
                   sigma_albedo=None if albedo is None else sa, moments=m, spp=spp, sigma_luminance=sl)
-    rc, o = mo.denoise(w, h, planes, desc, sl, spp, m, sa if albedo is not None else np.inf, albedo)
+    rc, o = mirrors.denoise(w, h, planes, desc, albedo, sa if albedo is not None else np.inf, moments=m, spp=spp, sigma_luminance=sl)
     assert rc == L.RAYN_OK and set(g) == set(o)
     for k in g:
         assert_bit_equal(g[k].reshape(-1), o[k], f"{what} {k}")
@@ -333,7 +333,7 @@ def test_variance_spaces_and_aliasing(renderer):
     w, h = 67, 45
     p, m = moment_film(w, h, 21)
     d = denoise_desc(5, 2.5, 0.4, 0.5)
-    rc, ref = mo.denoise(w, h, p, d, 2.0, 8, m)
+    rc, ref = mirrors.denoise(w, h, p, d, moments=m, spp=8, sigma_luminance=2.0)
     assert rc == L.RAYN_OK
     flat = {k: np.ascontiguousarray(v).reshape(-1) for k, v in p.items()}
     mflat = np.ascontiguousarray(m.transpose(2, 0, 1)).reshape(2, -1)
@@ -379,8 +379,8 @@ def test_film_moments_channel():
     moments = film.channels["moments"]
     film.denoise(3)
     from rayn_b200.film import DENOISE_LUMINANCE_SIGMA, DENOISE_VARIANCE_SIGMA_COLOR
-    rc, o = mo.denoise(48, 32, {**before, "normal": film.channels["normal"], "alpha": film.channels["alpha"]},
-                       denoise_desc(3, DENOISE_VARIANCE_SIGMA_COLOR), DENOISE_LUMINANCE_SIGMA, inp.spp, moments)
+    rc, o = mirrors.denoise(48, 32, {**before, "normal": film.channels["normal"], "alpha": film.channels["alpha"]},
+                            denoise_desc(3, DENOISE_VARIANCE_SIGMA_COLOR), moments=moments, spp=inp.spp, sigma_luminance=DENOISE_LUMINANCE_SIGMA)
     for k in COLOR_CH:
         assert_bit_equal(film.channels[k].reshape(-1), o[k], f"Film.denoise {k}")
     # the moments describe the unfiltered render: they leave with the first filter, and a second call is the unguided one

@@ -1,5 +1,5 @@
 """Motion against an explicit previous scene (rayn_b200_render_motion_prev, k_motion_paths_prev) on the device against its
-CPU mirror (tests/motion_prev_oracle.cpp) bit for bit: configs 1, 3 and 4, orthographic and thin-lens cameras, an orbit, a cut and
+CPU mirror (tests/render_mirror.cpp) bit for bit: configs 1, 3 and 4, orthographic and thin-lens cameras, an orbit, a cut and
 a zoom, limits_scenes.shape_c (15 moving spheres) with displaced previous centres and changed velocities, several passes,
 sampled tiles of a 1080p film, host and device planes, and the albedo plane of the same pass against render_albedo.  Also the
 identity with render_motion, the argument errors, Film.render_sequence on a world with closure parameters against the explicit
@@ -16,7 +16,7 @@ from rayn_b200.film import FrameInputs, Renderer, make_frame_desc
 from rayn_b200.scene import Linear, OrthographicCamera, PinholeCamera, Sphere, ThinLensCamera, Vec3
 
 import limits_scenes as ls
-import motion_prev_oracle as mpo
+import mirrors
 from helpers import assert_bit_equal, small_config
 from test_cpu_albedo import trap_config
 from test_cpu_motion_prev import changed_kind, rot_y
@@ -31,7 +31,7 @@ def both(r, world, cam, prev_desc, inp, tile, integ, albedo=False):
     """(device plane [, albedo], mirror plane) against prev_desc; the uploaded scene is world with cam"""
     d, keep = r.upload_scene(world, cam, TR)
     g = r.render_motion(inp, tile, integ, TR, DT, albedo=albedo, prev=prev_desc)
-    o = mpo.render_motion_prev(d, prev_desc, inp, tile, integ, TR, DT)[0]
+    o = mirrors.render_motion(d, inp, tile, integ, TR, DT, prev=prev_desc)[0]
     return g, o
 
 
@@ -126,7 +126,7 @@ def test_full_size_cfg3_sampled_tiles(renderer):
     d, keep = renderer.upload_scene(c["world"], cur, TR)
     p = c["world"].flatten(prv, TR)
     g = renderer.render_motion(inp, (16, 16), c["integrator"], TR, DT, prev=p[0])
-    o = mpo.render_motion_prev(d, p[0], inp, (16, 16), c["integrator"], TR, DT, subsample_k=97)[0]
+    o = mirrors.render_motion(d, inp, (16, 16), c["integrator"], TR, DT, prev=p[0], subsample_k=97)[0]
     nty = (1080 + 1080 % 16) // 16
     for t in range(0, 120 * nty, 97):
         tx, ty = t // nty, t % nty
@@ -148,7 +148,7 @@ def test_device_planes(renderer):
     torch.cuda.synchronize()
     L.check(renderer._lib.rayn_b200_render_motion_prev(renderer.ctx, C.byref(f), DT, C.byref(p[0]), m.data_ptr(), a.data_ptr(), L.MEM_DEVICE),
             renderer.ctx)
-    o = mpo.render_motion_prev(d, p[0], inp, (8, 8), c["integrator"], TR, DT)[0]
+    o = mirrors.render_motion(d, inp, (8, 8), c["integrator"], TR, DT, prev=p[0])[0]
     assert_bit_equal(m.cpu().numpy().reshape(19, 27, 4), o, "device motion")
     assert_bit_equal(a.cpu().numpy().reshape(19, 27, 3), renderer.render_albedo(inp, (8, 8), c["integrator"], TR), "device albedo")
 
@@ -260,7 +260,7 @@ def test_film_render_sequence_with_closures(shutter):
             assert_bit_equal(seen[i]["motion"], mv, f"frame {k} motion")
             assert_bit_equal(seen[i]["albedo"], alb, f"frame {k} albedo")
             if prev is not None:
-                o = mpo.render_motion_prev(scene[0], prev[0], g_inp, (16, 16), c["integrator"], tr, frame_dt)[0]
+                o = mirrors.render_motion(scene[0], g_inp, (16, 16), c["integrator"], tr, frame_dt, prev=prev[0])[0]
                 assert_bit_equal(mv, o, f"frame {k} motion mirror")
                 assert (np.abs(mv[..., 0][np.isfinite(mv[..., 2])]) > 0.1).mean() > 0.5  # the orbit moves the image
             prev = scene

@@ -1,6 +1,6 @@
 """Motion plane (rayn_b200_render_motion, rt_motion.cuh), temporal push (rayn_b200_temporal_push, rt_temporal.cuh) and the
 scaled variance denoise (rayn_b200_film_denoise_variance_scaled) on the device against their CPU mirrors
-(tests/motion_oracle.cpp, tests/temporal_oracle.cpp) bit for bit: configs 1, 3 and 4 (thin lens), an orthographic and a
+(tests/render_mirror.cpp, tests/film_mirror.cpp) bit for bit: configs 1, 3 and 4 (thin lens), an orthographic and a
 moving pinhole camera, 15 moving spheres, odd sizes, 8x8 and 16x16 tiles, several passes, sampled tiles of a 1080p film, the
 albedo plane of the same pass against render_albedo, exact zero motion on static scenes, a rendered camera-dolly sequence and a
 moving-sphere sequence through push (history ping-pong, reset, disocclusion, aliased planes, host and device planes) and the
@@ -16,8 +16,7 @@ from rayn_b200.film import FrameInputs, Renderer, denoise_desc
 from rayn_b200.scene import Linear, OrthographicCamera, PinholeCamera, Vec3
 
 import limits_scenes as ls
-import moments_oracle as mo
-import temporal_oracle as to
+import mirrors
 from helpers import assert_bit_equal, small_config
 from test_cpu_albedo import trap_config
 
@@ -33,7 +32,7 @@ def gpu_motion(r, c, inp, tile, camera=None, albedo=False):
 
 
 def mirror(c, inp, tile, camera=None, **kw):
-    return to.render_motion(c["world"], camera if camera is not None else c["camera"], inp, tile, c["integrator"], TR, DT, **kw)[0]
+    return mirrors.render_motion(c["world"].flatten(camera if camera is not None else c["camera"])[0], inp, tile, c["integrator"], TR, DT, **kw)[0]
 
 
 def dolly(c, res, speed=1.5):
@@ -74,7 +73,7 @@ def test_limits_shape_c_moving_spheres(renderer):
     integ, inp = ls.inputs((29, 21), 2, 1)
     renderer.upload_scene(world, cam)
     g = renderer.render_motion(inp, (8, 8), integ, TR, DT)
-    o = to.render_motion(world, cam, inp, (8, 8), integ, TR, DT)[0]
+    o = mirrors.render_motion(world.flatten(cam)[0], inp, (8, 8), integ, TR, DT)[0]
     assert_bit_equal(g, o, "shape C")
     assert (g[..., 0] != 0).any()
 
@@ -103,7 +102,7 @@ def test_full_size_cfg3_sampled_tiles(renderer):
     inp = FrameInputs(1920, 1080, 1, c["integrator"])
     cam = dolly(c, (1920, 1080))
     g = gpu_motion(renderer, c, inp, (16, 16), cam)
-    o = to.render_motion(c["world"], cam, inp, (16, 16), c["integrator"], TR, DT, subsample_k=97)[0]
+    o = mirrors.render_motion(c["world"].flatten(cam)[0], inp, (16, 16), c["integrator"], TR, DT, subsample_k=97)[0]
     nty = (1080 + 1080 % 16) // 16
     for t in range(0, 120 * nty, 97):
         tx, ty = t // nty, t % nty
@@ -168,7 +167,7 @@ def test_sequence_push_and_scaled_denoise(renderer, scene):
     frames = sequence(renderer, c, cam, res, 2, 6)
     kw = dict(alpha_min=0.2, sigma_depth=0.05, normal_cos=0.8)
     t = renderer.temporal_create(*res)
-    tm = to.TemporalMirror(*res)
+    tm = mirrors.TemporalMirror(*res)
     spp = 8
     d = denoise_desc(3, np.inf, 0.3, 0.2)
     try:
@@ -180,7 +179,7 @@ def test_sequence_push_and_scaled_denoise(renderer, scene):
                 assert (g[2] < 1).any()
             planes = dict(p, color=g[0]["color"], background=g[0]["background"])
             dn = renderer.denoise(res[0], res[1], planes, 3, np.inf, 0.3, 0.2, moments=g[1], spp=spp, sigma_luminance=4.0, var_scale=g[2])
-            rc, o = to.denoise_scaled(res[0], res[1], planes, d, 4.0, spp, g[1], g[2])
+            rc, o = mirrors.denoise(res[0], res[1], planes, d, moments=g[1], spp=spp, sigma_luminance=4.0, var_scale=g[2])
             assert rc == 0
             for ch in ("color", "background"):
                 assert_bit_equal(dn[ch], o[ch].reshape(dn[ch].shape), f"frame {k} denoise {ch}")
@@ -269,7 +268,7 @@ def test_pixel_without_a_hit_takes_no_history(renderer):
     """synthetic frames: a pixel whose motion is (0, 0, +inf, +inf) takes the current frame, on the device as in the mirror"""
     from test_cpu_temporal import frame
     w, h = 11, 8
-    t, tm = renderer.temporal_create(w, h), to.TemporalMirror(w, h)
+    t, tm = renderer.temporal_create(w, h), mirrors.TemporalMirror(w, h)
     try:
         for k, (p, m, mv) in enumerate([frame(w, h, 120), frame(w, h, 121, static=False)]):
             if k == 1:
@@ -312,8 +311,8 @@ def test_film_render_sequence(renderer, tmp_path):
                 assert_bit_equal(seen[i][ch], out[ch].reshape(res[1], res[0], 3), f"frame {k} {ch}")
             assert_bit_equal(seen[i]["motion"], mv, f"frame {k} motion")
             assert_bit_equal(seen[i]["albedo"], alb, f"frame {k} albedo")
-            assert_bit_equal(mv, to.render_motion(c["world"], cam, FrameInputs(res[0], res[1], 2, c["integrator"], frame=k), (16, 16),
-                                                  c["integrator"], tr, DT)[0], f"frame {k} motion mirror")
+            assert_bit_equal(mv, mirrors.render_motion(c["world"].flatten(cam)[0], FrameInputs(res[0], res[1], 2, c["integrator"], frame=k),
+                                                       (16, 16), c["integrator"], tr, DT)[0], f"frame {k} motion mirror")
     finally:
         t.close()
         r.close()

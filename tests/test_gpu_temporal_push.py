@@ -8,7 +8,7 @@ import pytest
 
 from rayn_b200 import _lib as L
 
-import temporal_oracle as to
+import mirrors
 import test_cpu_temporal_push as tp
 import test_cpu_temporal_reprojection as rp
 from helpers import assert_bit_equal
@@ -90,7 +90,7 @@ def test_edge_sequence_equals_the_mirror_with_an_overflowing_depth_test(renderer
     at every alpha_min and normal_cos of the CPU descriptors: device and mirror agree bit for bit on every output"""
     W, H = 37, 23
     rng = np.random.default_rng(17)
-    mirror = to.TemporalMirror(W, H)
+    mirror = mirrors.TemporalMirror(W, H)
     t = renderer.temporal_create(W, H)
     try:
         for k in range(2 * len(tp.DESCS)):

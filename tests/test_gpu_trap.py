@@ -1,5 +1,5 @@
 """Orbit-trap albedo on the device (rayn_b200_set_albedo_traps, k_normals<V, true>, the TRAP shading kernels) against the CPU
-trap oracle (tests/trap_oracle.cpp) bit for bit: the trap KAT, films at odd sizes and tile shapes, a material shared by a sphere
+trap oracle (tests/render_mirror.cpp) bit for bit: the trap KAT, films at odd sizes and tile shapes, a material shared by a sphere
 and the Mandelbox, sampled tiles of a full-size film, fold-all on and off, graph replay, pass sizes, host and device planes, the identity films, the
 golden fixture, the existing goldens after a clear, adaptive rounds and argument errors."""
 import ctypes as C

@@ -1,5 +1,5 @@
 """Orbit-trap distribution of config 3's first hits, on the CPU: pinhole camera rays through pixel centres, the render
-oracle's closest hit, then the trap oracle's trap (tests/trap_oracle.py) at every hit on the Mandelbox.  Its 5th and 95th
+oracle's closest hit, then the trap oracle's trap (tests/mirrors.py) at every hit on the Mandelbox.  Its 5th and 95th
 percentiles are the example trap range documented in the README and DESIGN.md §4d (TRAP_LO / TRAP_HI below, used by
 tools/bench_trap.py and the trap golden fixture).  Needs no GPU.
 
@@ -13,7 +13,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))  # the trap oracle (tests/trap_oracle.py) is test infrastructure
+sys.path.insert(0, os.path.join(ROOT, "tests"))  # the trap oracle (tests/mirrors.py) is test infrastructure
 
 # printed by this script for config 3 at 480x270, rounded (5th percentile 0.66756, 95th 1.45031; the fused mul_add oracle
 # agrees to 5 digits)
@@ -35,7 +35,7 @@ def camera_rays(cam, w, h):
 
 
 def first_hit_traps(config=3, res=(480, 270)):
-    import trap_oracle
+    import mirrors
     from oracle import binding as ob
     from rayn_b200 import _lib as L
     from rayn_b200 import configs
@@ -46,7 +46,7 @@ def first_hit_traps(config=3, res=(480, 270)):
     sdf = [i for i in range(desc.n_hitables) if desc.hitables[i].kind != L.HITABLE_SPHERE][0]
     hit = obj == sdf
     p = (d[hit] * t[hit, None] + o[hit]).astype(np.float32)
-    return trap_oracle.kat_sdf_trap(desc.hitables[sdf], p), hit.mean()
+    return mirrors.kat_sdf_trap(desc.hitables[sdf], p), hit.mean()
 
 
 def main():
