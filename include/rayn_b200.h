@@ -353,8 +353,8 @@ int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* fr
  * albedo[3p+c] = (((+0 + a_0[c]) + a_1[c]) + ... + a_{spp-1}[c]) / (float)spp, summed in ascending sample order; pixels
  * outside the tile grid are 0.  frame->tile_list / tile_offset / tile_stride are ignored (the whole grid is rendered); all
  * other frame checks are render_frame's.  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; replaces RaynStats
- * like a render (k_albedo_paths counts under RAYN_K_NORMALS, k_albedo_resolve under RAYN_K_RESOLVE); never captured into a
- * CUDA graph, and later renders are unaffected.
+ * like a render (k_first_hit_paths counts under RAYN_K_NORMALS, k_albedo_resolve under RAYN_K_RESOLVE); never captured
+ * into a CUDA graph, and later renders are unaffected.
  * Property (tested): if every Lambertian / Dielectric material has albedo (1, 1, 1) and there are no traps, every channel
  * equals render_frame's alpha plane bit for bit, for the same frame: alpha is nA / spp with nA the count of depth-0
  * Lambertian / Dielectric hits, and a sum of nA ones is nA exactly.                                                 */
@@ -385,7 +385,7 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, fl
  * Both projections are the same function, so a static camera and a static scene give dx = dy = +0 and z_prev == z exactly
  * (tested).  If albedo != NULL it is rayn_b200_render_albedo's plane for the same frame, bit for bit, from the same march.
  * frame_dt must be finite.  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; stats and graph rules are
- * rayn_b200_render_albedo's (k_motion_paths counts under RAYN_K_NORMALS, k_motion_resolve under RAYN_K_RESOLVE).          */
+ * rayn_b200_render_albedo's (k_first_hit_paths counts under RAYN_K_NORMALS, k_motion_resolve under RAYN_K_RESOLVE).       */
 int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* frame, float frame_dt, float* motion /* [4*W*H] */,
                                 float* albedo /* [3*W*H] or NULL */, int32_t space);
 
@@ -411,7 +411,7 @@ int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* frame, fl
  * RAYN_ERR_INVALID_ARG: prev NULL, prev->hitables NULL, a non-finite frame_dt, prev->n_hitables different from the uploaded
  * scene's, a hitable kind that differs, or a camera kind that differs (a cut to another camera type is a history reset, not
  * motion).  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; stats and graph rules are rayn_b200_render_motion's
- * (k_motion_paths_prev counts under RAYN_K_NORMALS).                                                                         */
+ * (k_first_hit_paths counts under RAYN_K_NORMALS).                                                                           */
 int32_t rayn_b200_render_motion_prev(RaynContext* ctx, const RaynFrameDesc* frame, float frame_dt, const RaynSceneDesc* prev,
                                      float* motion /* [4*W*H] */, float* albedo /* [3*W*H] or NULL */, int32_t space);
 

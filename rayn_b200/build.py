@@ -19,7 +19,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_build")
 OUT = os.path.join(OUT_DIR, "librayn_b200.so")
 SOURCES = [os.path.join(CSRC, "api.cu"), os.path.join(CSRC, "host_inputs.cpp")]
-DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("rt_kernels.cuh", "rt_device.cuh", "rt_sdf2.cuh", "rt_legacy.cuh", "rt_denoise.cuh", "rt_accum.cuh", "rt_albedo.cuh", "rt_motion.cuh", "rt_temporal.cuh", "detmath.h")] + [
+DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("rt_kernels.cuh", "rt_device.cuh", "rt_sdf2.cuh", "rt_legacy.cuh", "rt_denoise.cuh", "rt_accum.cuh", "rt_first_hit.cuh", "rt_temporal.cuh", "detmath.h")] + [
     os.path.join(HERE, "..", "include", "rayn_b200.h")]
 
 NVCC_FLAGS = [

@@ -14,10 +14,9 @@
 #include <vector>
 
 #include "rt_accum.cuh"
-#include "rt_albedo.cuh"
 #include "rt_denoise.cuh"
+#include "rt_first_hit.cuh"
 #include "rt_kernels.cuh"
-#include "rt_motion.cuh"
 #include "rt_temporal.cuh"
 #ifdef RAYN_LEGACY_KERNELS
 #include "rt_legacy.cuh"
@@ -68,6 +67,12 @@ struct PassBuf {
 };
 static const int N_PASS_BUFS = 23;
 
+// One host-space output plane of a job (job_stage): the caller's pointer (NULL: not asked for) and its floats per pixel.
+struct JobPlane {
+  float* user;
+  int floats;
+};
+
 struct RaynContext {
   int device = 0;
   int flags = 0;
@@ -94,8 +99,6 @@ struct RaynContext {
   size_t cap_s1 = 0, cap_s2 = 0, cap_scr = 0;
   float* d_planes = nullptr;
   size_t cap_planes = 0;
-  float* d_moments = nullptr;  // host-space moment planes of rayn_b200_render_frame_moments: 2 floats per pixel
-  size_t cap_moments = 0;
   int* d_pack_ids = nullptr;
   size_t cap_pack_ids = 0;
   unsigned char* d_post = nullptr;
@@ -111,6 +114,7 @@ struct RaynContext {
   // a render that has been enqueued but not finished
   bool pending = false;
   std::vector<int> job_tiles;
+  std::vector<JobPlane> job_out;  // the job's host-space outputs, staged back to back in d_planes in this order (job_stage)
   int job_w = 0, job_h = 0, job_tw = 0, job_th = 0, job_spp = 0, job_nty = 0;
   unsigned long long h_counters[CNT_TOTAL];
   RaynComm comm;
@@ -403,7 +407,6 @@ void rayn_b200_destroy(RaynContext* ctx) {
   cudaFree(ctx->d_pack_ids);
   cudaFree(ctx->d_post);
   cudaFree(ctx->d_s1), cudaFree(ctx->d_s2), cudaFree(ctx->d_scr), cudaFree(ctx->d_fis), cudaFree(ctx->d_planes);
-  cudaFree(ctx->d_moments);
   cudaFree(ctx->d_prev);
   for (auto& t : ctx->timed) cudaEventDestroy(t.a), cudaEventDestroy(t.b);
   if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
@@ -774,8 +777,9 @@ static int32_t job_begin(RaynContext* ctx, const RaynFrameDesc* f, const std::ve
   } else {
     for (int idx = f->tile_offset; idx < fr.ntx * fr.nty; idx += stride) my_tiles.push_back(idx);
   }
-  // the job's geometry, for render_finish once the caller has marked the job pending
+  // the job's geometry, for render_finish once the caller has marked the job pending; no host-space outputs until job_stage
   ctx->job_w = f->width, ctx->job_h = f->height, ctx->job_tw = f->tile_w, ctx->job_th = f->tile_h, ctx->job_spp = fr.spp, ctx->job_nty = fr.nty;
+  ctx->job_out.clear();
 
   memset(&ctx->stats, 0, sizeof ctx->stats);
   ctx->timed_used = 0;
@@ -799,6 +803,21 @@ static int32_t job_begin(RaynContext* ctx, const RaynFrameDesc* f, const std::ve
 static int32_t pass_tiles(RaynContext* ctx, Job* J, size_t first) {
   const int nt = J->pb.n_tiles = (int)std::min<size_t>(J->tiles_per_pass, ctx->job_tiles.size() - first);
   CU(cudaMemcpyAsync(ctx->d_tile_ids, ctx->job_tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  return RAYN_OK;
+}
+
+// Stages the job's n host-space outputs back to back in ctx->d_planes, in the order of `planes`, and zeroes the whole
+// staging if `zero`; stage[i] receives the staging of planes[i], also of a plane whose user pointer is NULL.  The offsets,
+// the staging size and job_end's copies all come from this one list.
+static int32_t job_stage(RaynContext* ctx, const JobPlane* planes, int n, bool zero, float** stage) {
+  const size_t npx = (size_t)ctx->job_w * ctx->job_h;
+  size_t floats = 0;
+  for (int i = 0; i < n; ++i) floats += planes[i].floats;
+  CU(regrow(&ctx->d_planes, &ctx->cap_planes, floats * npx));
+  if (zero) CU(cudaMemsetAsync(ctx->d_planes, 0, floats * npx * sizeof(float), ctx->stream));
+  floats = 0;
+  for (int i = 0; i < n; ++i) stage[i] = ctx->d_planes + floats * npx, floats += planes[i].floats;
+  ctx->job_out.assign(planes, planes + n);
   return RAYN_OK;
 }
 
@@ -831,35 +850,27 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, volume_on = P.volume_on;
   cudaStream_t st = ctx->stream;
 
+  if (mom && wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
   const size_t npx = (size_t)f->width * f->height;
   RaynFilmPlanes dp = *out;  // the device-space planes the film is rendered into
-  if (out->space == RAYN_MEM_HOST) {
-    CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 10));
-    CU(cudaMemsetAsync(ctx->d_planes, 0, npx * 10 * 4, st));
-    dp = film_block_planes(ctx->d_planes, npx);
+  float *dm_color = mom ? moments->color_lum2 : nullptr, *dm_bg = mom ? moments->background_lum2 : nullptr;  // ... and moment planes
+  if (out->space == RAYN_MEM_HOST) {  // (render_frame_moments: the moment planes are in out->space too)
+    // the film block (film_block_planes' layout), then with moments the two moment planes
+    const JobPlane planes[6] = {{out->color, 3}, {out->alpha, 1}, {out->background, 3}, {out->normal, 3}, {dm_color, 1}, {dm_bg, 1}};
+    float* stage[6];
+    if ((rc = job_stage(ctx, planes, mom ? 6 : 4, true, stage))) return rc;
+    dp = RaynFilmPlanes{stage[0], stage[1], stage[2], stage[3], RAYN_MEM_DEVICE};
+    dm_color = dm_color ? stage[4] : nullptr, dm_bg = dm_bg ? stage[5] : nullptr;
   } else {
     const int cov_w = std::min(fr.ntx * f->tile_w, f->width), cov_h = std::min(fr.nty * f->tile_h, f->height);
-    if (cov_w < f->width || cov_h < f->height)
+    if (cov_w < f->width || cov_h < f->height) {
       k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, dp.color, dp.alpha, dp.background, dp.normal);
+      for (float* m : {dm_color, dm_bg})  // the one-channel slot of k_zero_uncovered, once per plane
+        if (m) k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, nullptr, m, nullptr, nullptr);
+    }
   }
   dp.space = RAYN_MEM_DEVICE;
   if (dev_planes_out) *dev_planes_out = dp;
-  float *dm_color = nullptr, *dm_bg = nullptr;  // the device-space moment planes
-  if (mom) {
-    if (wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
-    if (moments->space == RAYN_MEM_HOST) {
-      CU(regrow(&ctx->d_moments, &ctx->cap_moments, npx * 2));
-      CU(cudaMemsetAsync(ctx->d_moments, 0, npx * 2 * 4, st));
-      dm_color = moments->color_lum2 ? ctx->d_moments : nullptr;
-      dm_bg = moments->background_lum2 ? ctx->d_moments + npx : nullptr;
-    } else {
-      dm_color = moments->color_lum2, dm_bg = moments->background_lum2;
-      const int cov_w = std::min(fr.ntx * f->tile_w, f->width), cov_h = std::min(fr.nty * f->tile_h, f->height);
-      if (cov_w < f->width || cov_h < f->height)  // the one-channel slot of k_zero_uncovered, once per plane
-        for (float* m : {dm_color, dm_bg})
-          if (m) k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, nullptr, m, nullptr, nullptr);
-    }
-  }
 
   const size_t res_smem = resolve_smem_per_warp(np, mom) * wpc;
   int slot_bits = 5, depth_bits = 1;  // significant bits of a shading slot (< QS) and of a depth (<= max_bounces): what k_resolve's radix sort walks
@@ -881,6 +892,9 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     key = fnv1a(1469598103934665603ull, &ctx->scene, sizeof ctx->scene);
     key = fnv1a(key, &fr, sizeof fr);
     key = fnv1a(key, &kpb, sizeof kpb);
+    // every plane pointer: host-space moment planes are staged after the film block, so the first such render may grow
+    // d_planes from 10 to 12 floats per pixel and move the film block; the moved pointers give a new key, and regrow only
+    // grows, so a graph is replayed only into the staging it was captured with
     float* planes6[6] = {dp.color, dp.alpha, dp.background, dp.normal, dm_color, dm_bg};
     key = fnv1a(key, planes6, sizeof planes6);
     const int misc[7] = {np, wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0, mom ? 1 : 0};  // mom: the k_resolve instance
@@ -1024,20 +1038,22 @@ static int32_t copy_planes(RaynContext* ctx, const RaynFilmPlanes& user, float* 
   return RAYN_OK;
 }
 
-// D2H of host-space planes (after an optional gather), then the end-of-frame bookkeeping
-static int32_t copy_out_enqueue(RaynContext* ctx, const RaynFilmPlanes* out) {
-  if (out->space != RAYN_MEM_HOST) return RAYN_OK;
-  return copy_planes(ctx, *out, ctx->d_planes, (size_t)ctx->job_w * ctx->job_h, cudaMemcpyDeviceToHost);
+// The D2H copies of the job's host-space outputs that the caller asked for, from their staging (job_stage).
+static int32_t copy_out(RaynContext* ctx) {
+  const size_t npx = (size_t)ctx->job_w * ctx->job_h;
+  const float* stage = ctx->d_planes;
+  for (const JobPlane& p : ctx->job_out) {
+    if (p.user) CU(cudaMemcpyAsync(p.user, stage, npx * p.floats * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    stage += npx * p.floats;
+  }
+  return RAYN_OK;
 }
 
-// D2H of host-space moment planes from their staging (ctx->d_moments: color_lum2, then background_lum2)
-static int32_t copy_moments_out(RaynContext* ctx, const RaynMomentPlanes* m) {
-  if (m->space != RAYN_MEM_HOST) return RAYN_OK;
-  const size_t npx = (size_t)ctx->job_w * ctx->job_h;
-  float* const dst[2] = {m->color_lum2, m->background_lum2};
-  for (int i = 0; i < 2; ++i)
-    if (dst[i]) CU(cudaMemcpyAsync(dst[i], ctx->d_moments + i * npx, npx * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  return RAYN_OK;
+// The tail of a pending job: copy_out unless rc is already an error, then render_finish even if that failed; the first error.
+static int32_t job_end(RaynContext* ctx, int32_t rc = RAYN_OK) {
+  if (!rc) rc = copy_out(ctx);
+  const int32_t rc2 = render_finish(ctx);
+  return rc ? rc : rc2;
 }
 
 static int32_t render_finish(RaynContext* ctx) {
@@ -1183,11 +1199,7 @@ int32_t rayn_b200_render_frame(RaynContext* ctx, const RaynFrameDesc* f, const R
   int32_t rc = check_planes(ctx, out, false);
   if (rc) return rc;
   if ((rc = render_enqueue(ctx, f, out, nullptr, nullptr))) return rc;
-  if ((rc = copy_out_enqueue(ctx, out))) {
-    render_finish(ctx);
-    return rc;
-  }
-  return render_finish(ctx);
+  return job_end(ctx);
 }
 
 // render_frame plus the lum^2 moment planes (statement in include/rayn_b200.h): the same job, with the k_resolve<true> instance
@@ -1201,66 +1213,16 @@ int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* f,
   if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
   int32_t rc = render_enqueue(ctx, f, out, nullptr, nullptr, moments);
   if (rc) return rc;
-  if ((rc = copy_out_enqueue(ctx, out)) || (rc = copy_moments_out(ctx, moments))) {
-    render_finish(ctx);
-    return rc;
-  }
-  return render_finish(ctx);
+  return job_end(ctx);
 }
 
-// The first-hit albedo plane (statement in include/rayn_b200.h): the render's raygen and depth-0 closest-hit stage, then
-// k_albedo_paths and k_albedo_resolve (rt_albedo.cuh), pass by pass over the whole tile grid.  Never captured into a graph.
-int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float* albedo, int32_t space) {
-  int32_t rc = job_ready(ctx, "render_albedo");
-  if (rc) return rc;
-  if (!f || !albedo) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/albedo is NULL");
-  if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_albedo: bad memory space %d", space);
-  if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_albedo: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)");
-  Job J;  // the render's own pass sizing: alternating renders and albedo passes reuse the same pass buffers
-  if ((rc = job_begin(ctx, f, nullptr, false, space, &J))) return rc;
-  const DevFrame& fr = J.P.fr;
-  const PassBufs& pb = J.pb;
-  cudaStream_t st = ctx->stream;
-  const size_t npx = (size_t)f->width * f->height;
-  float* dst = albedo;
-  if (space == RAYN_MEM_HOST) {
-    CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 3));
-    dst = ctx->d_planes;
-  }
-  CU(cudaMemsetAsync(dst, 0, npx * 3 * sizeof(float), st));  // pixels outside the tile grid stay 0
-  const Thr thr = make_thr(ctx->scene.cam, 0);
-  for (size_t first = 0; first < ctx->job_tiles.size(); first += J.tiles_per_pass) {
-    if ((rc = pass_tiles(ctx, &J, first))) return rc;
-    pass_raygen(ctx, J);
-    if ((rc = extend_enqueue(ctx, J, thr))) return rc;
-    timed_begin(ctx, RAYN_K_NORMALS);
-    k_albedo_paths<<<dim3((J.P.R + 255) / 256, pb.n_tiles), 256, 0, st>>>(ctx->scene, fr, pb, pb.nrm);
-    timed_end(ctx, RAYN_K_NORMALS);
-    timed_begin(ctx, RAYN_K_RESOLVE);
-    k_albedo_resolve<<<dim3((f->tile_w * f->tile_h + 255) / 256, pb.n_tiles), 256, 0, st>>>(fr, pb, pb.nrm, dst);
-    timed_end(ctx, RAYN_K_RESOLVE);
-    CU(cudaGetLastError());
-  }
-  ctx->pending = true;
-  if (space == RAYN_MEM_HOST) {
-    const cudaError_t e = cudaMemcpyAsync(albedo, dst, npx * 3 * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) {
-      render_finish(ctx);
-      CU(e);
-    }
-  }
-  return render_finish(ctx);
-}
-
-// The first-hit motion plane and optionally the albedo plane (statements in include/rayn_b200.h): the albedo pass's job with
-// k_motion_paths (prev == NULL) or k_motion_paths_prev and k_motion_resolve (rt_motion.cuh), and k_albedo_resolve on the same
-// per-path albedos.  Never captured.
-static int32_t motion_job(RaynContext* ctx, const char* name, const RaynFrameDesc* f, float frame_dt, bool use_prev,
-                          const RaynSceneDesc* prev, float* motion, float* albedo, int32_t space) {
-  int32_t rc = job_ready(ctx, name);
-  if (rc) return rc;
-  if (!f || !motion) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/motion is NULL");
-  if (use_prev && !prev) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: prev is NULL", name);
+// The first-hit passes (statements in include/rayn_b200.h): the albedo plane (motion == NULL), or the motion plane and
+// optionally the albedo plane, against the uploaded scene run backwards (prev == NULL) or against prev.  Each pass runs the
+// render's raygen and depth-0 closest-hit stage, then one k_first_hit_paths instance and the resolves (rt_first_hit.cuh),
+// pass by pass over the whole tile grid.  Never captured into a graph.  The callers have made job_ready and their own
+// pointer checks.
+static int32_t first_hit_job(RaynContext* ctx, const char* name, const RaynFrameDesc* f, float frame_dt, const RaynSceneDesc* prev,
+                             float* motion, float* albedo, int32_t space) {
   if (space != RAYN_MEM_HOST && space != RAYN_MEM_DEVICE) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: bad memory space %d", name, space);
   if (!isfinite(frame_dt)) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: frame_dt %g is not finite", name, frame_dt);
   if (ctx->flags & RAYN_FLAG_SIMPLE_MARCH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "%s: RAYN_FLAG_SIMPLE_MARCH (legacy test kernels)", name);
@@ -1285,65 +1247,70 @@ static int32_t motion_job(RaynContext* ctx, const char* name, const RaynFrameDes
       if (h.kind == RAYN_HITABLE_SPHERE && zero_v && memcmp(p.center, h.center, sizeof h.center) == 0) dp.still |= 1u << j;
     }
   }
-  Job J;
-  if ((rc = job_begin(ctx, f, nullptr, false, space, &J))) return rc;
+  Job J;  // the render's own pass sizing: alternating renders and first-hit passes reuse the same pass buffers
+  int32_t rc = job_begin(ctx, f, nullptr, false, space, &J);
+  if (rc) return rc;
   const DevFrame& fr = J.P.fr;
   const PassBufs& pb = J.pb;
   cudaStream_t st = ctx->stream;
   const size_t npx = (size_t)f->width * f->height;
-  float *dm_ = motion, *da = albedo;
+  float* dev[2] = {motion, albedo};  // the device-space planes: motion, then albedo, also in the host-space staging
   if (space == RAYN_MEM_HOST) {
-    CU(regrow(&ctx->d_planes, &ctx->cap_planes, npx * 7));
-    dm_ = ctx->d_planes, da = albedo ? ctx->d_planes + 4 * npx : nullptr;
+    const JobPlane planes[2] = {{motion, 4}, {albedo, 3}};
+    if ((rc = job_stage(ctx, planes, 2, false, dev))) return rc;
   }
+  float *dm = motion ? dev[0] : nullptr, *da = albedo ? dev[1] : nullptr;
   if (prev) {  // pageable source: the copy has left dp when cudaMemcpyAsync returns
     if (!ctx->d_prev) CU(cudaMalloc(&ctx->d_prev, sizeof(DevPrev)));
     CU(cudaMemcpyAsync(ctx->d_prev, &dp, sizeof dp, cudaMemcpyHostToDevice, st));
   }
-  k_motion_clear<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>((long long)npx, dm_);  // pixels outside the tile grid
-  if (da) CU(cudaMemsetAsync(da, 0, npx * 3 * sizeof(float), st));
+  if (dm) k_motion_clear<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>((long long)npx, dm);  // pixels outside the tile grid
+  if (da) CU(cudaMemsetAsync(da, 0, npx * 3 * sizeof(float), st));                          // ... which stay 0
+  typedef void (*PathsKernel)(DevScene, DevFrame, PassBufs, float, const DevPrev*);
+  static const PathsKernel motion_paths[2][2] = {  // [prev][albedo]
+      {k_first_hit_paths<true, false, false>, k_first_hit_paths<true, true, false>},
+      {k_first_hit_paths<true, false, true>, k_first_hit_paths<true, true, true>}};
+  const PathsKernel paths = dm ? motion_paths[prev != nullptr][da != nullptr] : k_first_hit_paths<false, true, false>;
   const Thr thr = make_thr(ctx->scene.cam, 0);
-  const dim3 paths_grid((J.P.R + 255) / 256, 1), pix_grid((f->tile_w * f->tile_h + 255) / 256, 1);
   for (size_t first = 0; first < ctx->job_tiles.size(); first += J.tiles_per_pass) {
     if ((rc = pass_tiles(ctx, &J, first))) return rc;
     pass_raygen(ctx, J);
     if ((rc = extend_enqueue(ctx, J, thr))) return rc;
-    const dim3 gp(paths_grid.x, pb.n_tiles), gr(pix_grid.x, pb.n_tiles);
+    const dim3 gp((J.P.R + 255) / 256, pb.n_tiles), gr((f->tile_w * f->tile_h + 255) / 256, pb.n_tiles);
     timed_begin(ctx, RAYN_K_NORMALS);
-    if (prev && da)
-      k_motion_paths_prev<true><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt, ctx->d_prev);
-    else if (prev)
-      k_motion_paths_prev<false><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt, ctx->d_prev);
-    else if (da)
-      k_motion_paths<true><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
-    else
-      k_motion_paths<false><<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt);
+    paths<<<gp, 256, 0, st>>>(ctx->scene, fr, pb, frame_dt, prev ? ctx->d_prev : nullptr);
     timed_end(ctx, RAYN_K_NORMALS);
     timed_begin(ctx, RAYN_K_RESOLVE);
-    k_motion_resolve<<<gr, 256, 0, st>>>(fr, pb, pb.rad, dm_);
+    if (dm) k_motion_resolve<<<gr, 256, 0, st>>>(fr, pb, pb.rad, dm);
     if (da) k_albedo_resolve<<<gr, 256, 0, st>>>(fr, pb, pb.nrm, da);
-    timed_end(ctx, RAYN_K_RESOLVE, da ? 2 : 1);
+    timed_end(ctx, RAYN_K_RESOLVE, (dm ? 1 : 0) + (da ? 1 : 0));
     CU(cudaGetLastError());
   }
   ctx->pending = true;
-  if (space == RAYN_MEM_HOST) {
-    cudaError_t e = cudaMemcpyAsync(motion, dm_, npx * 4 * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && albedo) e = cudaMemcpyAsync(albedo, da, npx * 3 * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) {
-      render_finish(ctx);
-      CU(e);
-    }
-  }
-  return render_finish(ctx);
+  return job_end(ctx);
+}
+
+int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* f, float* albedo, int32_t space) {
+  int32_t rc = job_ready(ctx, "render_albedo");
+  if (rc) return rc;
+  if (!f || !albedo) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/albedo is NULL");
+  return first_hit_job(ctx, "render_albedo", f, 0.0f, nullptr, nullptr, albedo, space);
 }
 
 int32_t rayn_b200_render_motion(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, float* motion, float* albedo, int32_t space) {
-  return motion_job(ctx, "render_motion", f, frame_dt, false, nullptr, motion, albedo, space);
+  int32_t rc = job_ready(ctx, "render_motion");
+  if (rc) return rc;
+  if (!f || !motion) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/motion is NULL");
+  return first_hit_job(ctx, "render_motion", f, frame_dt, nullptr, motion, albedo, space);
 }
 
 int32_t rayn_b200_render_motion_prev(RaynContext* ctx, const RaynFrameDesc* f, float frame_dt, const RaynSceneDesc* prev, float* motion,
                                      float* albedo, int32_t space) {
-  return motion_job(ctx, "render_motion_prev", f, frame_dt, true, prev, motion, albedo, space);
+  int32_t rc = job_ready(ctx, "render_motion_prev");
+  if (rc) return rc;
+  if (!f || !motion) return fail(ctx, RAYN_ERR_INVALID_ARG, "frame/motion is NULL");
+  if (!prev) return fail(ctx, RAYN_ERR_INVALID_ARG, "render_motion_prev: prev is NULL");
+  return first_hit_job(ctx, "render_motion_prev", f, frame_dt, prev, motion, albedo, space);
 }
 
 int32_t rayn_b200_sync(RaynContext* ctx) {
@@ -1426,10 +1393,7 @@ int32_t rayn_b200_render_frame_sharded(RaynContext* ctx, const RaynFrameDesc* f,
   const std::vector<int> tiles = shard_of(f->width, f->height, f->tile_w, f->tile_h, ctx->comm.rank, ctx->comm.world);
   RaynFilmPlanes dev;
   if ((rc = render_enqueue(ctx, f, out, &tiles, &dev))) return rc;
-  rc = gather_enqueue(ctx, f->width, f->height, f->tile_w, f->tile_h, &dev, false);
-  if (!rc) rc = copy_out_enqueue(ctx, out);
-  const int32_t rc2 = render_finish(ctx);
-  return rc ? rc : rc2;
+  return job_end(ctx, gather_enqueue(ctx, f->width, f->height, f->tile_w, f->tile_h, &dev, false));
 }
 
 int32_t rayn_b200_render_frame_multi(RaynContext* const* ctxs, int32_t n, const RaynFrameDesc* f, const RaynFilmPlanes* out) {
@@ -1472,10 +1436,9 @@ int32_t rayn_b200_render_frame_multi(RaynContext* const* ctxs, int32_t n, const 
       cudaSetDevice(ctxs[i]->device);
       first_err = gather_unpack(ctxs[i], &dev[i]);
     }
-    if (!first_err) first_err = copy_out_enqueue(ctx, out);
   }
-  for (int i = 0; i < n; ++i) {
-    const int32_t rc2 = render_finish(ctxs[i]);
+  for (int i = 0; i < n; ++i) {  // the caller's planes are copied from the first context's staging
+    const int32_t rc2 = i == 0 ? job_end(ctx, first_err) : render_finish(ctxs[i]);
     if (!first_err && rc2) first_err = rc2;
   }
   return first_err;

@@ -260,32 +260,34 @@ class Renderer:
     def render_albedo(self, inputs, tile_size, integrator, time_range):
         """First-hit albedo plane of the uploaded scene (include/rayn_b200.h: rayn_b200_render_albedo) for host FrameInputs:
         float32 [H, W, 3]."""
-        w, h = inputs.width, inputs.height
-        out = np.zeros(3 * w * h, np.float32)
-        ptrs = tuple(a.ctypes.data for a in inputs.arrays())
-        f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST,
-                            sets=(inputs.sets_1d, inputs.sets_2d))
-        L.check(self._lib.rayn_b200_render_albedo(self._ctx, C.byref(f), out.ctypes.data, L.MEM_HOST), self._ctx)
-        return out.reshape(h, w, 3)
+        return self._first_hit(inputs, tile_size, integrator, time_range, None, True, None)[1]
 
     def render_motion(self, inputs, tile_size, integrator, time_range, frame_dt, albedo=False, prev=None):
         """First-hit motion plane of the uploaded scene (include/rayn_b200.h: rayn_b200_render_motion) for host FrameInputs:
         float32 [H, W, 4] (dx, dy, z, z_prev); albedo=True: (motion, render_albedo's [H, W, 3] plane from the same pass).
         prev: the RaynSceneDesc the previous frame was rendered with (World.flatten's or upload_scene's, its keepalive still
         held): the motion against that scene instead of the uploaded one run backwards (rayn_b200_render_motion_prev)."""
+        motion, alb = self._first_hit(inputs, tile_size, integrator, time_range, frame_dt, albedo, prev)
+        return (motion, alb) if albedo else motion
+
+    def _first_hit(self, inputs, tile_size, integrator, time_range, frame_dt, albedo, prev):
+        """One first-hit pass: (motion [H, W, 4] or None, albedo [H, W, 3] or None).  frame_dt None: the albedo pass
+        (rayn_b200_render_albedo); else render_motion, or render_motion_prev against prev."""
         w, h = inputs.width, inputs.height
-        out = np.zeros(4 * w * h, np.float32)
-        alb = np.zeros(3 * w * h, np.float32) if albedo else None
+        motion = None if frame_dt is None else np.zeros((h, w, 4), np.float32)
+        alb = np.zeros((h, w, 3), np.float32) if albedo else None
         ptrs = tuple(a.ctypes.data for a in inputs.arrays())
         f = make_frame_desc(w, h, tile_size, inputs.samples, integrator, inputs.frame, time_range, ptrs, L.MEM_HOST,
                             sets=(inputs.sets_1d, inputs.sets_2d))
-        a_ptr = None if alb is None else alb.ctypes.data
-        if prev is None:
-            L.check(self._lib.rayn_b200_render_motion(self._ctx, C.byref(f), float(frame_dt), out.ctypes.data, a_ptr, L.MEM_HOST), self._ctx)
+        m_ptr, a_ptr = (None if a is None else a.ctypes.data for a in (motion, alb))
+        if frame_dt is None:
+            rc = self._lib.rayn_b200_render_albedo(self._ctx, C.byref(f), a_ptr, L.MEM_HOST)
+        elif prev is None:
+            rc = self._lib.rayn_b200_render_motion(self._ctx, C.byref(f), float(frame_dt), m_ptr, a_ptr, L.MEM_HOST)
         else:
-            L.check(self._lib.rayn_b200_render_motion_prev(self._ctx, C.byref(f), float(frame_dt), C.byref(prev), out.ctypes.data, a_ptr,
-                                                           L.MEM_HOST), self._ctx)
-        return (out.reshape(h, w, 4), alb.reshape(h, w, 3)) if albedo else out.reshape(h, w, 4)
+            rc = self._lib.rayn_b200_render_motion_prev(self._ctx, C.byref(f), float(frame_dt), C.byref(prev), m_ptr, a_ptr, L.MEM_HOST)
+        L.check(rc, self._ctx)
+        return motion, alb
 
     def temporal_create(self, width, height):
         return Temporal(self, width, height)

@@ -1,4 +1,4 @@
-"""First-hit albedo plane on the device (rayn_b200_render_albedo, rt_albedo.cuh) against its CPU mirror
+"""First-hit albedo plane on the device (rayn_b200_render_albedo, rt_first_hit.cuh) against its CPU mirror
 (tests/render_mirror.cpp) bit for bit, and the albedo-guided denoise (rayn_b200_film_denoise_albedo) against its mirror
 (tests/film_mirror.cpp): odd sizes and tile shapes with and without traps, a trap material shared by a sphere and the
 Mandelbox, fold-all on and off, moving spheres, thin-lens and orthographic cameras, sampled tiles of a full-size film, host and

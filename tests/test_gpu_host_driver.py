@@ -1,7 +1,8 @@
-"""The host scheduler of rayn_b200/csrc/api.cu (pass sizing, the pass loop, graph capture and replay, the albedo pass, an
-accumulator round) against RaynStats recorded from an earlier build: tests/golden/host_driver_stats.json, written by
-tests/golden/make_golden_stats.py.  Every case fixes max_paths_per_pass, so its pass size does not depend on the GPU's free
-memory; a change of pass sizing or of the launch sequence shows as a different pass or launch count."""
+"""The host scheduler of rayn_b200/csrc/api.cu (pass sizing, the pass loop, graph capture and replay, moment planes, the
+albedo and motion passes, an accumulator round) against RaynStats recorded from an earlier build:
+tests/golden/host_driver_stats.json, written by tests/golden/make_golden_stats.py.  Every case fixes max_paths_per_pass, so
+its pass size does not depend on the GPU's free memory; a change of pass sizing or of the launch sequence shows as a
+different pass or launch count."""
 import json
 import os
 
@@ -52,11 +53,11 @@ def with_renderer(max_paths, c, run):
         r.close()
 
 
-def render_case(c, inp, max_paths=MAX_PATHS, renders=1):
+def render_case(c, inp, max_paths=MAX_PATHS, renders=1, moments=False):
     def run(r):
         out = []
         for _ in range(renders):
-            r.render_host(inp, TILE, c["integrator"], TR)
+            r.render_host(inp, TILE, c["integrator"], TR, moments=moments)
             out.append(stats_fields(r))
         return out
     return with_renderer(max_paths, c, run)
@@ -67,6 +68,17 @@ def albedo_case():
 
     def run(r):
         r.render_albedo(inp, TILE, c["integrator"], TR)
+        return [stats_fields(r)]
+    return with_renderer(MAX_PATHS, c, run)
+
+
+def motion_case(albedo=False, prev=False):
+    """render_motion, or with prev render_motion_prev against the uploaded scene's own description"""
+    c, inp = trap_config(3)
+
+    def run(r):
+        desc = r.upload_scene(c["world"], c["camera"]) if prev else None
+        r.render_motion(inp, TILE, c["integrator"], TR, 0.5, albedo=albedo, prev=None if desc is None else desc[0])
         return [stats_fields(r)]
     return with_renderer(MAX_PATHS, c, run)
 
@@ -90,7 +102,13 @@ CASES = {
     "render_cfg3_trap_fold_all": lambda: render_case(*trap_config(3)),
     # a small single-pass frame: the first render captures the pass as a graph, the second replays it
     "render_cfg3_graph_replay": lambda: render_case(*small_config(3, (33, 27), 1, 3), max_paths=1 << 20, renders=2),
+    "render_moments_cfg3": lambda: render_case(*small_config(3, RES, 1, 3), moments=True),
+    "render_moments_cfg3_graph_replay": lambda: render_case(*small_config(3, (33, 27), 1, 3), max_paths=1 << 20, renders=2, moments=True),
     "render_albedo_cfg3_trap": albedo_case,
+    "render_motion_cfg3_trap": motion_case,
+    "render_motion_albedo_cfg3_trap": lambda: motion_case(albedo=True),
+    "render_motion_prev_cfg3_trap": lambda: motion_case(prev=True),
+    "render_motion_prev_albedo_cfg3_trap": lambda: motion_case(albedo=True, prev=True),
     "accum_round_cfg4": accum_case,
 }
 
@@ -107,7 +125,7 @@ def test_stats_equal_recorded(case):
         assert set(STRUCTURE) <= set(w), f"{case}: the fixture lacks structural fields"
         for k, v in w.items():
             assert g[k] == v, f"{case}, call {i}: {k} = {g[k]}, recorded {v}"
-    if case == "render_cfg3_graph_replay":
+    if case.endswith("graph_replay"):
         assert [g["reserved_"] for g in got] == [1, 1] and got[0]["passes"] == 1
     else:
         assert all(g["passes"] > 1 for g in got)

@@ -1,4 +1,4 @@
-"""Motion against an explicit previous scene (rayn_b200_render_motion_prev, k_motion_paths_prev) on the device against its
+"""Motion against an explicit previous scene (rayn_b200_render_motion_prev, k_first_hit_paths) on the device against its
 CPU mirror (tests/render_mirror.cpp) bit for bit: configs 1, 3 and 4, orthographic and thin-lens cameras, an orbit, a cut and
 a zoom, limits_scenes.shape_c (15 moving spheres) with displaced previous centres and changed velocities, several passes,
 sampled tiles of a 1080p film, host and device planes, and the albedo plane of the same pass against render_albedo.  Also the

@@ -1,4 +1,4 @@
-"""Motion plane (rayn_b200_render_motion, rt_motion.cuh), temporal push (rayn_b200_temporal_push, rt_temporal.cuh) and the
+"""Motion plane (rayn_b200_render_motion, rt_first_hit.cuh), temporal push (rayn_b200_temporal_push, rt_temporal.cuh) and the
 scaled variance denoise (rayn_b200_film_denoise_variance_scaled) on the device against their CPU mirrors
 (tests/render_mirror.cpp, tests/film_mirror.cpp) bit for bit: configs 1, 3 and 4 (thin lens), an orthographic and a
 moving pinhole camera, 15 moving spheres, odd sizes, 8x8 and 16x16 tiles, several passes, sampled tiles of a 1080p film, the
