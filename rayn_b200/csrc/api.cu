@@ -73,6 +73,18 @@ struct JobPlane {
   int floats;
 };
 
+// The state of one pass in flight: its buffers, the work counters of its persistent kernels and the stream it runs on.  A
+// render of several passes alternates them between two such sets, so that one pass's kernel tails, drains and single-CTA
+// scans overlap the other pass's work (render_enqueue).  The passes cover disjoint tiles and share only the stats counters.
+struct PassSet {
+  cudaStream_t stream = nullptr;      // set 0: the context's stream
+  size_t cap[N_PASS_BUFS] = {};       // bytes allocated per pass_table entry
+  PassBufs pb;                        // pb.counters: the context's stats counters, shared by both sets
+  int* d_tile_ids = nullptr;
+  int* d_batch_prefix = nullptr;  // [tiles per pass + 1]
+  int* d_work_ctr = nullptr;      // [WC_TOTAL] global work counters of the persistent kernels
+};
+
 struct RaynContext {
   int device = 0;
   int flags = 0;
@@ -81,12 +93,9 @@ struct RaynContext {
   bool has_scene = false;
   DevScene scene;
   int64_t cap_paths = 0;  // requested paths per pass
-  // pass buffers
-  size_t pass_cap[N_PASS_BUFS] = {};  // bytes allocated per pass_table entry
-  PassBufs pb;
-  int* d_tile_ids = nullptr;
-  int* d_batch_prefix = nullptr;  // [tiles per pass + 1]
-  int* d_work_ctr = nullptr;      // [WC_TOTAL] global work counters of the persistent kernels
+  PassSet ps[2];          // pass buffers; ps[1] only for renders of several passes (size_pass)
+  unsigned long long* d_counters = nullptr;  // [CNT_TOTAL] stats counters of the job, order-free atomics
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;  // ps[1].stream forks from and joins back into the context's stream
   int n_sm = 148;
   int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT], occ_nrm_trap[SDFV_COUNT];  // occ_ext[constant threshold][variant]
   int occ_pre = 8, occ_post = 8, occ_sph = 8;  // resident CTAs per SM of the work-list kernels
@@ -171,7 +180,7 @@ static cudaError_t regrow(T** p, size_t* cap, size_t need) {
 
 // Every pass buffer, in allocation order.  seg_per_path: shadow segments per path and depth over all SDF queues; lc_ns: light
 // samples per path and depth; trap: the scene has orbit-trap albedos (PassBufs::trap_s).
-static std::array<PassBuf, N_PASS_BUFS> pass_table(RaynContext* c, int QS, int seg_per_path, int lc_ns, bool trap) {
+static std::array<PassBuf, N_PASS_BUFS> pass_table(PassSet* c, int QS, int seg_per_path, int lc_ns, bool trap) {
   PassBufs& p = c->pb;
   const size_t nseg = (QS + SEG_SLOTS - 1) / SEG_SLOTS;  // segments per tile of the queue kernels
   return {{
@@ -201,51 +210,57 @@ static std::array<PassBuf, N_PASS_BUFS> pass_table(RaynContext* c, int QS, int s
   }};
 }
 
-static void free_pass(RaynContext* c) {
-  for (const PassBuf& b : pass_table(c, 0, 0, 0, false)) {
+static void free_pass(PassSet* s) {
+  for (const PassBuf& b : pass_table(s, 0, 0, 0, false)) {
     cudaFree(*b.ptr);
     *b.ptr = nullptr;
   }
-  unsigned long long* counters = c->pb.counters;
-  memset(&c->pb, 0, sizeof c->pb);
-  c->pb.counters = counters;
-  memset(c->pass_cap, 0, sizeof c->pass_cap);
+  unsigned long long* counters = s->pb.counters;
+  memset(&s->pb, 0, sizeof s->pb);
+  s->pb.counters = counters;
+  memset(s->cap, 0, sizeof s->cap);
+}
+
+static size_t pass_set_bytes(const PassSet& s) {
+  size_t bytes = 0;
+  for (size_t b : s.cap) bytes += b;
+  return bytes;
 }
 
 // bytes of pass state per path (what ensure_pass allocates, less the per-tile buffers), used to size passes against free
 // device memory
-static size_t pass_bytes_per_path(RaynContext* c, int R, int QS, int seg_per_path, int lc_ns, bool trap) {
+static size_t pass_bytes_per_path(PassSet* s, int R, int QS, int seg_per_path, int lc_ns, bool trap) {
   size_t bytes = 0;
-  for (const PassBuf& b : pass_table(c, QS, seg_per_path, lc_ns, trap))
+  for (const PassBuf& b : pass_table(s, QS, seg_per_path, lc_ns, trap))
     bytes += b.per_path + (b.per_slot ? (size_t)(((double)QS / R) * b.per_slot + 1) : 0);
   return bytes;
 }
 
-static int32_t ensure_pass(RaynContext* ctx, int n_tiles, int R, int QS, int seg_per_path, int n_sdf, int lc_ns, bool trap) {
+static int32_t ensure_pass(RaynContext* ctx, PassSet* s, int n_tiles, int R, int QS, int seg_per_path, int n_sdf, int lc_ns, bool trap) {
   const int64_t need_paths = (int64_t)n_tiles * R, need_q = (int64_t)n_tiles * QS;
-  const std::array<PassBuf, N_PASS_BUFS> table = pass_table(ctx, QS, seg_per_path, lc_ns, trap);
+  const std::array<PassBuf, N_PASS_BUFS> table = pass_table(s, QS, seg_per_path, lc_ns, trap);
   size_t need[N_PASS_BUFS];
   bool fits = true;
   for (int i = 0; i < N_PASS_BUFS; ++i) {
     const PassBuf& b = table[i];
     need[i] = b.per_path * need_paths + b.per_slot * need_q + b.per_tile * n_tiles + b.fixed;
-    fits = fits && need[i] <= ctx->pass_cap[i];
+    fits = fits && need[i] <= s->cap[i];
   }
   if (fits) return RAYN_OK;
-  free_pass(ctx);
+  free_pass(s);
   for (int i = 0; i < N_PASS_BUFS; ++i) {
     if (need[i] == 0) continue;
     const cudaError_t e = cudaMalloc(table[i].ptr, need[i]);
     if (e != cudaSuccess) {
       cudaGetLastError();
-      free_pass(ctx);
+      free_pass(s);
       return fail(ctx, e == cudaErrorMemoryAllocation ? RAYN_ERR_OOM : RAYN_ERR_CUDA, "pass buffers (%lld paths): %s", (long long)need_paths,
                   cudaGetErrorString(e));
     }
-    ctx->pass_cap[i] = need[i];
+    s->cap[i] = need[i];
   }
-  ctx->pb.prefix_stride = n_tiles + 1;
-  ctx->pb.seg_cap = n_sdf > 0 ? need_paths * seg_per_path / n_sdf : 0;
+  s->pb.prefix_stride = n_tiles + 1;
+  s->pb.seg_cap = n_sdf > 0 ? need_paths * seg_per_path / n_sdf : 0;
   return RAYN_OK;
 }
 
@@ -346,17 +361,24 @@ int32_t rayn_b200_create(const RaynConfig* cfg, RaynContext** out_ctx) {
   ctx->device = dev;
   ctx->flags = cfg ? cfg->flags : 0;
   ctx->cap_paths = (cfg && cfg->max_paths_per_pass > 0) ? cfg->max_paths_per_pass : (int64_t)96 << 20;  // fewer passes = fewer kernel tails; clamped to free memory per frame
-  memset(&ctx->pb, 0, sizeof ctx->pb);
   memset(&ctx->stats, 0, sizeof ctx->stats);
   memset(&ctx->scene, 0, sizeof ctx->scene);
   cudaError_t e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->pb.counters, CNT_TOTAL * sizeof(unsigned long long));
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->ps[1].stream, cudaStreamNonBlocking);
+  ctx->ps[0].stream = ctx->stream;
+  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_counters, CNT_TOTAL * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&ctx->d_fis, RAYN_FIS_TABLE_SIZE * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_work_ctr, WC_TOTAL * sizeof(int));
+  for (PassSet& s : ctx->ps) {
+    memset(&s.pb, 0, sizeof s.pb);
+    s.pb.counters = ctx->d_counters;
+    if (e == cudaSuccess) e = cudaMalloc(&s.d_work_ctr, WC_TOTAL * sizeof(int));
+  }
   if (e == cudaSuccess) e = cudaMalloc(&ctx->d_kat, sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx->n_sm, cudaDevAttrMultiProcessorCount, dev);
   if (e == cudaSuccess) e = cudaEventCreate(&ctx->ev0);
   if (e == cudaSuccess) e = cudaEventCreate(&ctx->ev1);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming);
   // persistent kernels: exactly as many CTAs as can be resident (one wave), so every CTA pulls work until the pass is drained
   for (int v = 0; v < SDFV_COUNT && e == cudaSuccess; ++v) {
     DISPATCH_SDFV(v, e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_ext[0][v], k_extend_march<V, false>, EXT_T, 0);
@@ -374,9 +396,10 @@ int32_t rayn_b200_create(const RaynConfig* cfg, RaynContext** out_ctx) {
     cudaGetLastError();
     fail(nullptr, RAYN_ERR_CUDA, "context setup: %s", cudaGetErrorString(e));
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    cudaFree(ctx->pb.counters), cudaFree(ctx->d_fis), cudaFree(ctx->d_work_ctr), cudaFree(ctx->d_kat);
-    if (ctx->ev0) cudaEventDestroy(ctx->ev0);
-    if (ctx->ev1) cudaEventDestroy(ctx->ev1);
+    if (ctx->ps[1].stream) cudaStreamDestroy(ctx->ps[1].stream);
+    cudaFree(ctx->d_counters), cudaFree(ctx->d_fis), cudaFree(ctx->ps[0].d_work_ctr), cudaFree(ctx->ps[1].d_work_ctr), cudaFree(ctx->d_kat);
+    for (cudaEvent_t ev : {ctx->ev0, ctx->ev1, ctx->ev_fork, ctx->ev_join})
+      if (ev) cudaEventDestroy(ev);
     delete ctx;
     return RAYN_ERR_CUDA;
   }
@@ -399,10 +422,13 @@ void rayn_b200_destroy(RaynContext* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
+  cudaStreamSynchronize(ctx->ps[1].stream);
   rayn_b200_comm_destroy(ctx);
-  free_pass(ctx);
-  cudaFree(ctx->pb.counters);
-  cudaFree(ctx->d_work_ctr);
+  for (PassSet& s : ctx->ps) {
+    free_pass(&s);
+    cudaFree(s.d_work_ctr);
+  }
+  cudaFree(ctx->d_counters);
   cudaFree(ctx->d_kat);
   cudaFree(ctx->d_pack_ids);
   cudaFree(ctx->d_post);
@@ -410,8 +436,8 @@ void rayn_b200_destroy(RaynContext* ctx) {
   cudaFree(ctx->d_prev);
   for (auto& t : ctx->timed) cudaEventDestroy(t.a), cudaEventDestroy(t.b);
   if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
-  cudaEventDestroy(ctx->ev0), cudaEventDestroy(ctx->ev1);
-  cudaStreamDestroy(ctx->stream);
+  cudaEventDestroy(ctx->ev0), cudaEventDestroy(ctx->ev1), cudaEventDestroy(ctx->ev_fork), cudaEventDestroy(ctx->ev_join);
+  cudaStreamDestroy(ctx->stream), cudaStreamDestroy(ctx->ps[1].stream);
   delete ctx;
 }
 
@@ -572,6 +598,11 @@ struct Job {
   FramePlan P;
   PassBufs pb;  // pb.n_tiles: the tiles of the current pass
   int tiles_per_pass;
+  int n_sets;   // pass sets in flight: 2 when the passes alternate between ctx->ps[0] and ctx->ps[1] (size_pass)
+  bool paired;  // the current pass runs beside a pass of the other set (march_grid)
+  // the current pass's set: its stream and the work lists and work counters of its persistent kernels
+  cudaStream_t st;
+  int *batch_prefix, *work_ctr;
 };
 
 // The resident grid (one wave) of a kernel that strides over a work list of the pass (k_scan_slots / k_scan_live), capped
@@ -680,36 +711,77 @@ static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
 }
 
 // Pass size for n_tiles tiles (as many tiles per pass as the path budget and free device memory allow), and the pass buffers.
-static int32_t size_pass(RaynContext* ctx, const FramePlan& P, size_t n_tiles, int* out_tiles_per_pass) {
+// A job that needs several passes sizes each from half the memory budget, so that two passes fit at once; with two_sets
+// (a render that may overlap its passes) it then also gets the second pass set, and *out_sets is 2.  A job that fits one
+// pass, a half budget that holds no tile, or a second set that does not fit leave one set, sized as for a single stream.
+static int32_t size_pass(RaynContext* ctx, const FramePlan& P, size_t n_tiles, bool two_sets, int* out_tiles_per_pass, int* out_sets) {
   const int R = P.R, QS = P.QS, n_sdf = ctx->scene.n_sdf, ns = P.ns, seg_per_path = P.seg_per_path, lc_ns = P.lc_ns;
   const bool traps = P.traps;
-  const size_t bpp = pass_bytes_per_path(ctx, R, QS, seg_per_path, lc_ns, traps);
-  size_t free_b = 0, total_b = 0, pass_bytes = 0;
+  const size_t bpp = pass_bytes_per_path(&ctx->ps[0], R, QS, seg_per_path, lc_ns, traps);
+  size_t free_b = 0, total_b = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
-  for (size_t b : ctx->pass_cap) pass_bytes += b;
-  const size_t budget = (size_t)((double)(free_b + pass_bytes) * 0.90);
-  int64_t max_paths = std::min<int64_t>(ctx->cap_paths, (int64_t)(budget / bpp));
-  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, ((int64_t)1 << 27) - 1);          // owner path index is packed with the sample bit (<< 4)
-  if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, (int64_t)INT_MAX / std::max(ns, 1));  // 32-bit queue cursors per SDF
+  const size_t budget = (size_t)((double)(free_b + pass_set_bytes(ctx->ps[0]) + pass_set_bytes(ctx->ps[1])) * 0.90);
+  auto tiles_for = [&](size_t bytes) {  // whole tiles of a pass that fits `bytes` (0: not even one)
+    int64_t max_paths = std::min<int64_t>(ctx->cap_paths, (int64_t)(bytes / bpp));
+    if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, ((int64_t)1 << 27) - 1);          // owner path index is packed with the sample bit (<< 4)
+    if (n_sdf > 0) max_paths = std::min<int64_t>(max_paths, (int64_t)INT_MAX / std::max(ns, 1));  // 32-bit queue cursors per SDF
+    return std::min<int64_t>(max_paths / R, 65535);
+  };
+  int64_t tiles = tiles_for(budget);
+  const bool several = tiles < (int64_t)n_tiles, halves = several && tiles_for(budget / 2) >= 1;
+  if (halves) tiles = tiles_for(budget / 2);
   int& tiles_per_pass = *out_tiles_per_pass;
-  tiles_per_pass = (int)std::max<int64_t>(1, max_paths / R);
-  tiles_per_pass = std::min(tiles_per_pass, 65535);
+  tiles_per_pass = (int)std::max<int64_t>(1, tiles);
   tiles_per_pass = std::min<int>(tiles_per_pass, (int)std::max<size_t>(n_tiles, 1));
   int32_t rc;
-  while ((rc = ensure_pass(ctx, tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps)) == RAYN_ERR_OOM && tiles_per_pass > 1)
+  while ((rc = ensure_pass(ctx, &ctx->ps[0], tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps)) == RAYN_ERR_OOM) {
+    if (pass_set_bytes(ctx->ps[1])) {  // the second set's memory goes first
+      free_pass(&ctx->ps[1]);
+      continue;
+    }
+    if (tiles_per_pass == 1) break;
     tiles_per_pass = (tiles_per_pass + 1) / 2;  // fragmentation / another tenant: retry with half the pass
+  }
+  *out_sets = 1;
+  if (rc || !two_sets || !halves || (size_t)tiles_per_pass >= n_tiles) return rc;
+  rc = ensure_pass(ctx, &ctx->ps[1], tiles_per_pass, R, QS, seg_per_path, n_sdf, lc_ns, traps);
+  if (rc == RAYN_ERR_OOM) return RAYN_OK;  // one pass at a time (ensure_pass left ps[1] empty)
+  if (rc == RAYN_OK) {
+    *out_sets = 2;
+    // passes of equal size (the same count), so that the two streams run their passes side by side to the end
+    const size_t passes = (n_tiles + tiles_per_pass - 1) / tiles_per_pass;
+    tiles_per_pass = (int)((n_tiles + passes - 1) / passes);
+  }
   return rc;
+}
+
+// Points J's current pass at pass set `set`: its buffers, stream, work lists and work counters.
+static void pass_set_use(RaynContext* ctx, Job* J, int set) {
+  PassSet& s = ctx->ps[set];
+  PassBufs& pb = J->pb = s.pb;
+  pb.R = J->P.R, pb.QS = J->P.QS, pb.tile_ids = s.d_tile_ids;
+  pb.lc_ns = J->P.lc_ns;
+  pb.seg_count = s.d_work_ctr + WC_SEG_COUNT;
+  J->st = s.stream, J->batch_prefix = s.d_batch_prefix, J->work_ctr = s.d_work_ctr;
+}
+
+// The grid of a persistent march (k_extend_march, k_shadow): one resident wave of occ CTAs per SM, or half of it while two
+// passes are in flight (J.paired).  Two marches then run side by side within one wave, and the other pass's short kernels (scans,
+// bins, shading, compaction) find free CTA slots at once instead of waiting for this march's drain.  Either way the march's
+// CTAs only take work from a global counter, so the grid size changes the schedule, never the result.
+static unsigned march_grid(const RaynContext* ctx, const Job& J, int occ) {
+  return (unsigned)ctx->n_sm * (J.paired ? (occ + 1) / 2 : occ);
 }
 
 // One depth's closest-hit stage (the non-legacy kernels): k_scan_live, then the fold over the live rays of the pass.
 static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
-  cudaStream_t st = ctx->stream;
+  cudaStream_t st = J.st;
   const PassBufs& pb = J.pb;
   const int n_hit = ctx->scene.n_hit, fold_pre = J.P.fold_pre;
   const bool fold_all = J.P.fold_all, motion = ctx->scene.sph_moving != 0;
   const unsigned sph_grid = resident(ctx, J, ctx->occ_sph);
   timed_begin(ctx, RAYN_K_MISC);
-  k_scan_live<<<1, SCAN_T, 0, st>>>(pb, ctx->d_batch_prefix, ctx->d_work_ctr);
+  k_scan_live<<<1, SCAN_T, 0, st>>>(pb, J.batch_prefix, J.work_ctr);
   timed_end(ctx, RAYN_K_MISC);
   // fold order of hitable.rs:177-198: runs of spheres as coherent kernels, each SDF as a persistent march.  The
   // spheres before the first SDF were already folded in by the kernel that produced the rays (fold_pre >= 0).
@@ -719,19 +791,19 @@ static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
     while (e < n_hit && ctx->scene.hit[e].kind == RAYN_HITABLE_SPHERE) ++e;
     if ((e > k || first_kernel) && !fold_all) {
       timed_begin(ctx, RAYN_K_EXTEND_SPHERES);
-      k_extend_spheres<<<sph_grid, EXT_BATCH, 0, st>>>(ctx->scene, pb, k, e, first_kernel, motion ? 1 : 0, ctx->d_batch_prefix, ctx->d_work_ctr + WC_SPHERES + k);
+      k_extend_spheres<<<sph_grid, EXT_BATCH, 0, st>>>(ctx->scene, pb, k, e, first_kernel, motion ? 1 : 0, J.batch_prefix, J.work_ctr + WC_SPHERES + k);
       timed_end(ctx, RAYN_K_EXTEND_SPHERES);
       first_kernel = 0;
     }
     if (e < n_hit) {
-      if (n_march++ > 0) CU(cudaMemsetAsync(ctx->d_work_ctr + WC_EXTEND, 0, sizeof(int), st));
+      if (n_march++ > 0) CU(cudaMemsetAsync(J.work_ctr + WC_EXTEND, 0, sizeof(int), st));
       const int v = ctx->sdf_var[e];
       timed_begin(ctx, RAYN_K_EXTEND);
       const int sf = fold_all ? 1 : 0;
       if (thr.is_const)
-        DISPATCH_SDFV(v, (k_extend_march<V, true><<<ctx->n_sm * ctx->occ_ext[1][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
+        DISPATCH_SDFV(v, (k_extend_march<V, true><<<march_grid(ctx, J, ctx->occ_ext[1][v]), EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
       else
-        DISPATCH_SDFV(v, (k_extend_march<V, false><<<ctx->n_sm * ctx->occ_ext[0][v], EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, ctx->d_batch_prefix, ctx->d_work_ctr + WC_EXTEND)))
+        DISPATCH_SDFV(v, (k_extend_march<V, false><<<march_grid(ctx, J, ctx->occ_ext[0][v]), EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
       timed_end(ctx, RAYN_K_EXTEND);
       ++e;
     }
@@ -789,20 +861,22 @@ static int32_t job_begin(RaynContext* ctx, const RaynFrameDesc* f, const std::ve
   CU(cudaEventRecord(ctx->ev0, ctx->stream));
   if ((rc = upload_tables(ctx, f, &P.fr))) return rc;
   if ((rc = scene_plan(ctx, &P))) return rc;
-  if ((rc = size_pass(ctx, P, my_tiles.size(), &J->tiles_per_pass))) return rc;
-  PassBufs& pb = J->pb = ctx->pb;
-  pb.R = P.R, pb.QS = P.QS, pb.tile_ids = ctx->d_tile_ids;
-  pb.lc_ns = P.lc_ns;
-  pb.seg_count = ctx->d_work_ctr + WC_SEG_COUNT;
-  CU(cudaMemsetAsync(pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), ctx->stream));
+  // Two passes in flight only for a render whose launches are not bracketed one by one (RAYN_FLAG_TIMING) and whose
+  // depths are not read back (the debug queue log)
+  const bool two_sets = render && !(ctx->flags & RAYN_FLAG_TIMING) && !ctx->qlog_enabled;
+  if ((rc = size_pass(ctx, P, my_tiles.size(), two_sets, &J->tiles_per_pass, &J->n_sets))) return rc;
+  pass_set_use(ctx, J, 0);
+  J->paired = false;
+  CU(cudaMemsetAsync(ctx->d_counters, 0, CNT_TOTAL * sizeof(unsigned long long), ctx->stream));
   return RAYN_OK;
 }
 
-// Starts the pass over tiles [first, first + tiles_per_pass) of the job: uploads their ids.  The upload reads host memory,
-// so a render's graph capture begins after it.
-static int32_t pass_tiles(RaynContext* ctx, Job* J, size_t first) {
+// Starts the pass over tiles [first, first + tiles_per_pass) of the job on pass set `set`: uploads their ids.  The upload
+// reads host memory, so a render's graph capture begins after it.
+static int32_t pass_tiles(RaynContext* ctx, Job* J, size_t first, int set) {
+  pass_set_use(ctx, J, set);
   const int nt = J->pb.n_tiles = (int)std::min<size_t>(J->tiles_per_pass, ctx->job_tiles.size() - first);
-  CU(cudaMemcpyAsync(ctx->d_tile_ids, ctx->job_tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->ps[set].d_tile_ids, ctx->job_tiles.data() + first, nt * sizeof(int), cudaMemcpyHostToDevice, J->st));
   return RAYN_OK;
 }
 
@@ -825,7 +899,7 @@ static int32_t job_stage(RaynContext* ctx, const JobPlane* planes, int n, bool z
 static void pass_raygen(RaynContext* ctx, const Job& J) {
   ctx->stats.passes++;
   timed_begin(ctx, RAYN_K_RAYGEN);
-  k_raygen<<<dim3((J.P.R + 255) / 256, J.pb.n_tiles), 256, 0, ctx->stream>>>(ctx->scene, J.P.fr, J.pb, J.P.n_fold);
+  k_raygen<<<dim3((J.P.R + 255) / 256, J.pb.n_tiles), 256, 0, J.st>>>(ctx->scene, J.P.fr, J.pb, J.P.n_fold);
   timed_end(ctx, RAYN_K_RAYGEN);
 }
 
@@ -848,7 +922,6 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   const int mb = fr.max_bounces, np = P.np, wpc = mom ? resolve_warps_per_cta(np, true) : P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
   const int* sdf_idx = ctx->scene.sdf_idx;
   const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, volume_on = P.volume_on;
-  cudaStream_t st = ctx->stream;
 
   if (mom && wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
   const size_t npx = (size_t)f->width * f->height;
@@ -864,9 +937,9 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   } else {
     const int cov_w = std::min(fr.ntx * f->tile_w, f->width), cov_h = std::min(fr.nty * f->tile_h, f->height);
     if (cov_w < f->width || cov_h < f->height) {
-      k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, dp.color, dp.alpha, dp.background, dp.normal);
+      k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(f->width, f->height, cov_w, cov_h, dp.color, dp.alpha, dp.background, dp.normal);
       for (float* m : {dm_color, dm_bg})  // the one-channel slot of k_zero_uncovered, once per plane
-        if (m) k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(f->width, f->height, cov_w, cov_h, nullptr, m, nullptr, nullptr);
+        if (m) k_zero_uncovered<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(f->width, f->height, cov_w, cov_h, nullptr, m, nullptr, nullptr);
     }
   }
   dp.space = RAYN_MEM_DEVICE;
@@ -901,15 +974,36 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     key = fnv1a(key, misc, sizeof misc);
     key = fnv1a(key, my_tiles.data(), my_tiles.size() * sizeof(int));
     if (ctx->graph_exec && ctx->graph_key == key) {
-      CU(cudaMemcpyAsync(ctx->d_tile_ids, my_tiles.data(), my_tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-      CU(cudaGraphLaunch(ctx->graph_exec, st));
+      CU(cudaMemcpyAsync(ctx->ps[0].d_tile_ids, my_tiles.data(), my_tiles.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+      CU(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
       ctx->stats = ctx->graph_stats;
       replayed = true;
     }
   }
+  // Several passes alternate between the two pass sets, pass k on set k % 2 and its stream: each stream runs its passes in
+  // order, so a set is reused only after its previous pass, and the two streams overlap one pass's tails with the other's
+  // work.  ps[1].stream starts after everything the job has enqueued so far and is joined back into the context's stream
+  // when the passes are enqueued, also on an error return, so whatever follows on the context's stream (copy-out, gather,
+  // render_finish, the accumulator fold, the next job) sees the whole film.
+  struct Join {
+    RaynContext* ctx;
+    bool on;
+    ~Join() {
+      if (on && cudaEventRecord(ctx->ev_join, ctx->ps[1].stream) == cudaSuccess) cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0);
+    }
+  } join{ctx, false};
+  if (J.n_sets > 1 && !replayed) {
+    CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
+    CU(cudaStreamWaitEvent(ctx->ps[1].stream, ctx->ev_fork, 0));
+    join.on = true;
+  }
   std::vector<int> h_nslots, h_slots;
-  for (size_t first = 0; first < my_tiles.size() && !replayed; first += J.tiles_per_pass) {
-    if ((rc = pass_tiles(ctx, &J, first))) return rc;
+  const size_t n_passes = (my_tiles.size() + J.tiles_per_pass - 1) / J.tiles_per_pass;
+  for (size_t first = 0, k = 0; first < my_tiles.size() && !replayed; first += J.tiles_per_pass, ++k) {
+    if ((rc = pass_tiles(ctx, &J, first, (int)(k % J.n_sets)))) return rc;
+    // the last pass of an odd count runs alone once its partner's pass ends: full waves
+    J.paired = J.n_sets > 1 && !(n_passes % 2 == 1 && k == n_passes - 1);
+    const cudaStream_t st = J.st;
     if (use_graph) {
       CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
       capturing = true;
@@ -955,30 +1049,30 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           const int v = ctx->sdf_var[sdf_idx[j]];
           timed_begin(ctx, RAYN_K_NORMALS);
           if ((ctx->scene.trap_mask >> h.material) & 1u)  // the bin's material has an orbit-trap albedo: normals + trap
-            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx, J, ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
+            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx, J, ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, J.work_ctr + WC_NORMALS + j)))
           else
-            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx, J, ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, ctx->d_work_ctr + WC_NORMALS + j)))
+            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx, J, ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, J.work_ctr + WC_NORMALS + j)))
           timed_end(ctx, RAYN_K_NORMALS);
         }
         timed_begin(ctx, RAYN_K_SHADE_PRE);
         if (traps)
-          k_shade_pre<true><<<resident(ctx, J, ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+          k_shade_pre<true><<<resident(ctx, J, ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
         else
-          k_shade_pre<false><<<resident(ctx, J, ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, ctx->d_work_ctr + WC_PRE);
+          k_shade_pre<false><<<resident(ctx, J, ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
         timed_end(ctx, RAYN_K_SHADE_PRE);
         if (ctx->scene.n_lights > 0) {
           for (int j = 0; j < n_sdf; ++j) {
             const int v = ctx->sdf_var[sdf_idx[j]];
             timed_begin(ctx, RAYN_K_SHADOW);
-            DISPATCH_SDFV(v, (k_shadow<V><<<ctx->n_sm * ctx->occ_shd[v], SHD_T, 0, st>>>(ctx->scene, pb, sdf_idx[j], j, ctx->d_work_ctr + WC_SHADOW + j)));
+            DISPATCH_SDFV(v, (k_shadow<V><<<march_grid(ctx, J, ctx->occ_shd[v]), SHD_T, 0, st>>>(ctx->scene, pb, sdf_idx[j], j, J.work_ctr + WC_SHADOW + j)));
             timed_end(ctx, RAYN_K_SHADOW);
           }
         }
         timed_begin(ctx, RAYN_K_SHADE_POST);
         if (traps)
-          k_shade_post<true><<<resident(ctx, J, ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+          k_shade_post<true><<<resident(ctx, J, ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);
         else
-          k_shade_post<false><<<resident(ctx, J, ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, ctx->d_work_ctr + WC_POST);
+          k_shade_post<false><<<resident(ctx, J, ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);
         timed_end(ctx, RAYN_K_SHADE_POST);
       } else {
 #ifdef RAYN_LEGACY_KERNELS
@@ -1062,7 +1156,7 @@ static int32_t render_finish(RaynContext* ctx) {
   cudaStream_t st = ctx->stream;
   CU(cudaSetDevice(ctx->device));
   CU(cudaEventRecord(ctx->ev1, st));
-  CU(cudaMemcpyAsync(ctx->h_counters, ctx->pb.counters, sizeof ctx->h_counters, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(ctx->h_counters, ctx->d_counters, sizeof ctx->h_counters, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   CU(cudaEventElapsedTime(&ctx->stats.total_ms, ctx->ev0, ctx->ev1));
@@ -1273,7 +1367,7 @@ static int32_t first_hit_job(RaynContext* ctx, const char* name, const RaynFrame
   const PathsKernel paths = dm ? motion_paths[prev != nullptr][da != nullptr] : k_first_hit_paths<false, true, false>;
   const Thr thr = make_thr(ctx->scene.cam, 0);
   for (size_t first = 0; first < ctx->job_tiles.size(); first += J.tiles_per_pass) {
-    if ((rc = pass_tiles(ctx, &J, first))) return rc;
+    if ((rc = pass_tiles(ctx, &J, first, 0))) return rc;
     pass_raygen(ctx, J);
     if ((rc = extend_enqueue(ctx, J, thr))) return rc;
     const dim3 gp((J.P.R + 255) / 256, pb.n_tiles), gr((f->tile_w * f->tile_h + 255) / 256, pb.n_tiles);
