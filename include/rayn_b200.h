@@ -664,7 +664,7 @@ int32_t rayn_b200_host_tile_grid(int32_t width, int32_t height, int32_t tile_w, 
 
 /* ---- kernel-level known-answer entry points (device execution, host pointers) -------
  * Used by tests to compare single stages against the oracle lane by lane.              */
-/* op: 0 exp, 1 ln, 2 pow(a,b), 3 sin, 4 cos, 5 tan, 6 atan2(a,b), 7 powi5               */
+/* op: 0 exp, 1 ln, 2 pow(a,b), 3 sin, 4 cos, 5 tan, 6 atan2(a,b), 7 powi5, 8 ln_fast    */
 int32_t rayn_b200_kat_detmath(RaynContext* ctx, int32_t op, int64_t n, const float* a,
                               const float* b, float* out);
 /* SDF::dist (sdf.rs:125-141) */
@@ -680,6 +680,11 @@ int32_t rayn_b200_kat_sdf_trap(RaynContext* ctx, const RaynHitable* sdf, int64_t
 /* Newton division of the Mandelbox sphere fold vs IEEE division: number of x among the n consecutive floats starting
  * at bit pattern first_bits for which num / x differs (must be 0 wherever the fast variants are selected)           */
 int32_t rayn_b200_kat_fastdiv(RaynContext* ctx, float num, uint32_t first_bits, int64_t n, int64_t* out_mismatches);
+/* detmath op (as kat_detmath) at every 32-bit pattern v as its first operand, b the second (swap != 0: b first, v second),
+ * inputs generated on the device: out_hashes256[c] = sum over the v with v >> 24 == c of
+ * splitmix64(((uint64_t)v << 32) | bits of the result)  mod 2^64; a NaN of powi5 counts as 0x7fc00000 (its payload is
+ * the hardware's, detmath.h)                                                                                          */
+int32_t rayn_b200_kat_detmath_sweep(RaynContext* ctx, int32_t op, float b, int32_t swap, uint64_t* out_hashes256);
 /* TracedSDF::hit (sdf.rs:59-83).  thr(t) = thr_scale * t, or thr_scale if thr_const != 0 */
 int32_t rayn_b200_kat_sdf_hit(RaynContext* ctx, const RaynHitable* sdf,
                               const RaynRenderConsts* consts, int64_t n, const float* origins3,

@@ -1197,6 +1197,7 @@ int32_t rayn_oracle_kat_detmath(int32_t op, int64_t n, const float* a, const flo
       case 5: out[i] = dm::tan(a[i]); break;
       case 6: out[i] = dm::atan2(a[i], b[i]); break;
       case 7: out[i] = dm::powi5(a[i]); break;
+      case 8: out[i] = dm::ln_fast(a[i]); break;
       default: return RAYN_ERR_INVALID_ARG;
     }
   }

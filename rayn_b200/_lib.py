@@ -150,6 +150,7 @@ SYMBOLS = {
     "rayn_b200_set_albedo_traps": (i32, [C.c_void_p, i32, C.POINTER(RaynAlbedoTrap)]),
     "rayn_b200_kat_sdf_trap": (i32, [C.c_void_p, C.POINTER(RaynHitable), i64, fp, fp]),
     "rayn_b200_kat_fastdiv": (i32, [C.c_void_p, f32, C.c_uint32, i64, C.POINTER(i64)]),
+    "rayn_b200_kat_detmath_sweep": (i32, [C.c_void_p, i32, f32, i32, C.POINTER(C.c_uint64)]),
     "rayn_b200_create": (i32, [C.POINTER(RaynConfig), C.POINTER(C.c_void_p)]),
     "rayn_b200_destroy": (None, [C.c_void_p]),
     "rayn_b200_last_error": (C.c_char_p, [C.c_void_p]),

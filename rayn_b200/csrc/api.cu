@@ -2059,7 +2059,7 @@ int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTem
 
 int32_t rayn_b200_kat_detmath(RaynContext* ctx, int32_t op, int64_t n, const float* a, const float* b, float* out) {
   KAT_PROLOGUE
-  if (op < 0 || op > 7 || !a || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_detmath: bad argument");
+  if (op < 0 || op > 8 || !a || !out) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_detmath: bad argument");
   float* da = tmp.up(a, n, &e);
   float* db = tmp.up(b ? b : a, n, &e);
   float* dout = tmp.up<float>(nullptr, n, &e);
@@ -2115,6 +2115,18 @@ int32_t rayn_b200_kat_fastdiv(RaynContext* ctx, float num, uint32_t first_bits, 
   CU(cudaMemcpyAsync(&h, ctx->d_kat, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   *out_mismatches = (int64_t)h;
+  return RAYN_OK;
+}
+int32_t rayn_b200_kat_detmath_sweep(RaynContext* ctx, int32_t op, float b, int32_t swap, uint64_t* out_hashes256) {
+  if (!ctx || op < 0 || op > 8 || !out_hashes256) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_detmath_sweep: bad argument");
+  CU(cudaSetDevice(ctx->device));
+  DevTmp tmp;
+  cudaError_t e = cudaSuccess;
+  unsigned long long* dh = tmp.up<unsigned long long>(nullptr, 256, &e);
+  CU(e);
+  CU(cudaMemsetAsync(dh, 0, 256 * sizeof(unsigned long long), ctx->stream));
+  k_kat_detmath_sweep<<<256 * KAT_SWEEP_BLOCKS, 256, 0, ctx->stream>>>(op, b, swap, dh);
+  KAT_EPILOGUE(out_hashes256, dh, 256, unsigned long long)
   return RAYN_OK;
 }
 int32_t rayn_b200_kat_sdf_hit(RaynContext* ctx, const RaynHitable* sdf, const RaynRenderConsts* consts, int64_t n, const float* origins3,

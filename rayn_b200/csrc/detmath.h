@@ -261,17 +261,11 @@ DM_HD float ln(float x) {
   return (float)ln_core((double)x);
 }
 
-// Float-only natural log (no double pipe): ~2e-7 relative accuracy.  Used by the AUTHORED
-// Mandelbulb distance estimator, whose definition is ours to make; bit-identical host/device
-// because it is built from IEEE float + - * / and integer bit operations only.
-DM_HD float ln_fast(float x) {
-  if (x != x) return x;
-  if (x < 0.0f) return u2f(0x7fc00000u);
-  if (x == 0.0f) return u2f(0xff800000u);
-  const uint32_t b = f2u(x);
-  if (b == 0x7f800000u) return x;
-  int e = (int)(b >> 23) - 127;
-  float m = u2f((b & 0x007fffffu) | 0x3f800000u);  // [1, 2)
+// ln of 2^((b >> 23) - 127) * 1.m, m the low 23 bits of b: a positive normal float's bit pattern, or a subnormal's
+// normalised one (exponent field below 1, so b >> 23 is negative)
+DM_HD float ln_fast_bits(int32_t b) {
+  int e = (b >> 23) - 127;
+  float m = u2f(((uint32_t)b & 0x007fffffu) | 0x3f800000u);  // [1, 2)
   if (m > 1.41421356f) {
     m = m * 0.5f;
     e = e + 1;
@@ -285,9 +279,34 @@ DM_HD float ln_fast(float x) {
   p = dfma(p, z, 1.0f);
   return (float)e * 0.693147180559945f + 2.0f * s * p;
 }
+// Float-only natural log (no double pipe): ~2e-7 relative accuracy.  Used by the AUTHORED
+// Mandelbulb distance estimator, whose definition is ours to make; bit-identical host/device
+// because it is built from IEEE float + - * / and integer bit operations only.
+DM_HD float ln_fast(float x) {
+  if (x != x) return x;
+  if (x < 0.0f) return u2f(0x7fc00000u);
+  const int32_t b = (int32_t)f2u(x);
+  if (b < 0x00800000) {  // +-0 (-0 has the sign bit) or subnormal: an early return, so the march loop's path is unchanged
+    if (x == 0.0f) return u2f(0xff800000u);
+    return ln_fast_bits((int32_t)f2u(x * 0x1p23f) - (23 << 23));  // x * 2^23 is exact and normal
+  }
+  if (b == 0x7f800000) return x;
+  return ln_fast_bits(b);
+}
 
-// powf for the domain the render path uses (x >= 0); negative base -> NaN like a
-// non-integer exponent would give.
+// ---- documented domain restrictions: where the functions below differ from C99 Annex F --------------------------
+// Everything else matches Annex F for zeros, subnormals, infinities and NaN (tests/test_cpu_shared_numerics.py
+// checks the full table of special operands on host and device and pins each value listed here).  These stay
+// because pow and sincos/tan sit on the shading path and no render reaches these operands:
+//   pow(x, y), x < 0 (-inf included), y != 0:   NaN     (C99: x^y for integer y, e.g. pow(-2, 2) = 4)
+//   pow(-0, y), y an odd integer:                +0 for y > 0, +inf for y < 0   (C99: -0, -inf)
+//   pow(1, NaN):                                 NaN     (C99: 1)
+//   sin, cos, tan of |x| > 1e5:                  NaN     (C99: finite)
+// NaN payloads: exp, ln and ln_fast return a NaN input as it is; pow, sin, cos, tan and atan2 return 0x7fc00000.
+// powi5 is plain float multiplies, so its NaN is the hardware's: the input's, quieted, on x86; 0x7fffffff on the GPU.
+// The measured accuracy over every float is in oracle/README.md (A9).
+
+// powf for the domain the render path uses (x >= 0).
 DM_HD float pow(float x, float y) {
   if (y == 0.0f) return 1.0f;
   if (x != x || y != y) return u2f(0x7fc00000u);
@@ -321,19 +340,21 @@ DM_HD float tan(float x) {
   return (float)(sd / cd);
 }
 
+// C99 Annex F atan2, signed zeros and infinite operands included: the quadrant follows the SIGN BITS, so
+// atan2(+-0, -0) = +-pi and atan2(-0, x > 0) = -0; |y| = |x| = inf gives +-pi/4 or +-3pi/4.
 DM_HD float atan2(float y, float x) {
   if (x != x || y != y) return u2f(0x7fc00000u);
   double ax = (double)dm::abs(x), ay = (double)dm::abs(y);
   double a;
-  if (ax == 0.0 && ay == 0.0) {
-    a = 0.0;
-  } else if (ay > ax) {
+  if (ay > ax) {
     a = DM_PIO2 - atan01_core(ax / ay);
+  } else if (ay == 0.0) {
+    a = 0.0;
   } else {
-    a = atan01_core(ay / ax);
+    a = atan01_core(ay == ax ? 1.0 : ay / ax);  // ay / ax = 1 for finite ties; inf / inf would be NaN
   }
-  if (x < 0.0f) a = DM_PI - a;
-  if (y < 0.0f) a = -a;
+  if (f2u(x) >> 31) a = DM_PI - a;
+  if (f2u(y) >> 31) a = -a;
   return (float)a;
 }
 

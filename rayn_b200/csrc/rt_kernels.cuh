@@ -1544,20 +1544,44 @@ __global__ void __launch_bounds__(256) k_gen_scramble(int W, int H, float* __res
 // ------------------------------------------------------------------------------------------
 // known-answer kernels (tests only)
 // ------------------------------------------------------------------------------------------
+RT_D float kat_detmath_op(int op, float a, float b) {
+  float s, c;
+  switch (op) {
+    case 0: return dm::exp(a);
+    case 1: return dm::ln(a);
+    case 2: return dm::pow(a, b);
+    case 3: dm::sincos(a, &s, &c); return s;
+    case 4: dm::sincos(a, &s, &c); return c;
+    case 5: return dm::tan(a);
+    case 6: return dm::atan2(a, b);
+    case 7: return dm::powi5(a);
+    default: return dm::ln_fast(a);
+  }
+}
 __global__ void k_kat_detmath(int op, long long n, const float* a, const float* b, float* out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float s, c;
-  switch (op) {
-    case 0: out[i] = dm::exp(a[i]); break;
-    case 1: out[i] = dm::ln(a[i]); break;
-    case 2: out[i] = dm::pow(a[i], b[i]); break;
-    case 3: dm::sincos(a[i], &s, &c); out[i] = s; break;
-    case 4: dm::sincos(a[i], &s, &c); out[i] = c; break;
-    case 5: out[i] = dm::tan(a[i]); break;
-    case 6: out[i] = dm::atan2(a[i], b[i]); break;
-    case 7: out[i] = dm::powi5(a[i]); break;
+  out[i] = kat_detmath_op(op, a[i], b[i]);
+}
+// every 32-bit pattern v as the first operand (the second with swap; b is the other): hash[v >> 24] += splitmix64((v << 32) | out bits),
+// mod 2^64 (tests/detmath_sweep.cpp sums the same on the host).  Grid: KAT_SWEEP_BLOCKS blocks per 2^24-pattern chunk.
+#define KAT_SWEEP_BLOCKS 64
+__global__ void __launch_bounds__(256) k_kat_detmath_sweep(int op, float b, int swap, unsigned long long* __restrict__ hash) {
+  const unsigned chunk = blockIdx.x / KAT_SWEEP_BLOCKS, per_block = (1u << 24) / KAT_SWEEP_BLOCKS;
+  const unsigned first = (chunk << 24) + (blockIdx.x % KAT_SWEEP_BLOCKS) * per_block;
+  unsigned long long h = 0;
+  for (unsigned k = threadIdx.x; k < per_block; k += blockDim.x) {
+    const unsigned v = first + k;
+    const float x = __uint_as_float(v);
+    const float out = swap ? kat_detmath_op(op, b, x) : kat_detmath_op(op, x, b);
+    const unsigned bits = op == 7 && out != out ? 0x7fc00000u : __float_as_uint(out);  // powi5's NaN payload is the hardware's
+    unsigned long long z = (((unsigned long long)v << 32) | bits) + 0x9e3779b97f4a7c15ull;  // splitmix64
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    h += z ^ (z >> 31);
   }
+  for (int o = 16; o > 0; o >>= 1) h += __shfl_down_sync(0xffffffffu, h, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(hash + chunk, h);
 }
 __global__ void k_kat_sdf_dist(const RaynHitable h, long long n, const float* p3, float* out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;

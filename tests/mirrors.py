@@ -21,6 +21,7 @@ COMMON = ["-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math
 RENDER = ("render_mirror", [os.path.join(HERE, "render_mirror.cpp"), os.path.join(ROOT, "oracle", "rayn_oracle.cpp")] + HEADERS,
           ["-O3", "-msse4.1", "-mavx2", "-mfma", "-fopenmp"] + COMMON)
 FILM = ("film_mirror", [os.path.join(HERE, "film_mirror.cpp")] + HEADERS, ["-O2"] + COMMON)
+SWEEP = ("detmath_sweep", [os.path.join(HERE, "detmath_sweep.cpp")] + HEADERS, RENDER[2])
 N_HIST = 14  # history planes of a RaynTemporal
 fp = C.POINTER(C.c_float)
 P = C.POINTER
@@ -78,6 +79,41 @@ def film_lib():
         l.rayn_oracle_exp.argtypes = [C.c_float]
         _libs["film"] = l
     return _libs["film"]
+
+
+class SweepAcc(C.Structure):
+    _fields_ = [("max_err", C.c_double), ("argmax", C.c_uint32), ("over", C.c_int64)]
+
+
+def sweep_lib():
+    if "sweep" not in _libs:
+        l = _build(*SWEEP)
+        l.detmath_sweep.restype = C.c_int32
+        l.detmath_sweep.argtypes = [C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, P(C.c_uint64),
+                                    P(SweepAcc)]
+        l.detmath_error.restype = C.c_double
+        l.detmath_error.argtypes = [C.c_int32, C.c_float, C.c_float, C.c_float]
+        _libs["sweep"] = l
+    return _libs["sweep"]
+
+
+def detmath_sweep(op, fixed, swap, chunk0, n_chunks, accuracy, bound):
+    """tests/detmath_sweep.cpp over chunks [chunk0, chunk0 + n_chunks) -> (hashes [n_chunks] uint64, None or
+    ({"max", "argmax", "over"} over the contract domain, the same over the render-path domain))"""
+    hashes = np.zeros(n_chunks, np.uint64)
+    acc = (SweepAcc * 2)()
+    rc = sweep_lib().detmath_sweep(op, float(fixed), 1 if swap else 0, chunk0, n_chunks, 1 if accuracy else 0, float(bound),
+                                   hashes.ctypes.data_as(P(C.c_uint64)), acc)
+    if rc != 0:
+        raise ValueError(f"detmath_sweep: bad argument (op {op}, chunks {chunk0}+{n_chunks})")
+    if not accuracy:
+        return hashes, None
+    return hashes, tuple({"max": a.max_err, "argmax": a.argmax, "over": a.over} for a in acc)
+
+
+def detmath_error(op, a, b, got):
+    """the sweep's error measure of one result against long-double libm (ulp; relative for ln_fast, op 8)"""
+    return sweep_lib().detmath_error(op, float(a), float(b), float(got))
 
 
 def _f(a):
