@@ -138,8 +138,25 @@ typedef struct RaynLight {
 typedef enum RaynCameraKind {
   RAYN_CAMERA_PINHOLE = 0,     /* src/camera.rs:42-119  */
   RAYN_CAMERA_THINLENS = 1,    /* src/camera.rs:121-213 */
-  RAYN_CAMERA_ORTHOGRAPHIC = 2 /* src/camera.rs:215-285 */
+  RAYN_CAMERA_ORTHOGRAPHIC = 2, /* src/camera.rs:215-285 */
+  RAYN_CAMERA_EQUIRECTANGULAR = 3 /* EXTENSION, no reference counterpart: a 360-degree panorama, below */
 } RaynCameraKind;
+
+/* ---- equirectangular (360-degree panorama) camera: an EXTENSION with no reference counterpart ----------------------------
+ * Reads origin, at, up and their velocities (the same lane-0-time closure semantics as the other kinds) and half_pixel_size,
+ * which the host sets to the angular half pixel (pi_f / (float)H) / 2.0f, in float, so the depth-0 hit threshold
+ * half_pixel_size * t is the half pixel's arc at distance t.  Every other field is ignored.  With pi_f = 3.14159265f and
+ * 2pi_f = 6.28318531f (the floats nearest pi and 2 pi), in float with the build's mul_add (dot / cross / normalized as the
+ * other cameras):
+ *   bw = normalized(origin - at),  bu = normalized(cross(up, bw)),  bv = cross(bw, bu)      (the pinhole basis)
+ *   phi = (u - 0.5f) * 2pi_f,  theta = (v - 0.5f) * pi_f,  (sp, cp) = dm::sincos(phi),  (st, ct) = dm::sincos(theta)
+ *   rd = normalized((bu * (ct * sp) + bv * st) - bw * (ct * cp)),  ro = origin
+ * (vector * scalar per component, each operation rounded on its own).  The screen centre looks at `at`, +u turns towards bu,
+ * v = 1 is the `up` pole.  A filter offset that pushes u outside [0, 1] wraps round the seam, since sin and cos are periodic.
+ * Column 0 and column W-1 are neighbours: rayn_b200_film_denoise_wrap and rayn_b200_temporal_push_wrap filter such a film.
+ * The one trap: the tile grid of film.rs:399-404 drops the last partial tile when 0 < W % tile_w < tile_w / 2, which leaves
+ * those columns black at the seam.  The ABI keeps the reference grid; the Python Film and rayn_host refuse such widths for a
+ * panorama.                                                                                                                   */
 
 /* The derived fields are what the reference constructors store (camera.rs:52-72,
  * 133-157,227-241); the HOST computes them (tan etc. are host-side f32 libm there too),
@@ -376,10 +393,16 @@ int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, fl
  *        py = ((dot(r, bv) / (z * hy)) * 0.5f + 0.5f) * (float)H
  *     orthographic: bw = normalized(at - origin), bu = normalized(cross(bw, up)), bv = cross(bu, bw), z = dot(r, bw),
  *        px = ((dot(r, bu) + hx) / full_size[0]) * (float)W, py = ((dot(r, bv) + hy) / full_size[1]) * (float)H
+ *     equirectangular: the pinhole basis, xr = dot(r, bu), yr = dot(r, bv), zr = -dot(r, bw), z = mag(r) (the distance:
+ *        the temporal depth test is relative, so distance serves it), px = (dm::atan2(xr, zr) / 2pi_f + 0.5f) * (float)W,
+ *        py = (dm::atan2(yr, sqrtf(xr*xr + zr*zr)) / pi_f + 0.5f) * (float)H, the products of the sqrt's argument rounded
+ *        on their own
  *     (hx, hy = half_size): the inverse of camera_ray's pixel -> (u, v) map, px = u * W, in film pixels
  *   (px1, py1, z)      = proj(P, tau),  (px0, py0, z_prev) = proj(P', tau - frame_dt)
- *   the sample is VALID if it hit something and, for a pinhole / thin-lens camera, z > 0 and z_prev > 0; its record is
- *   (px0 - px1, py0 - py1, z, z_prev), and an invalid sample's record is (0, 0, NaN, NaN) (so a NaN z also counts invalid).
+ *   the sample is VALID if it hit something and, for a pinhole / thin-lens / equirectangular camera, z > 0 and z_prev > 0; its
+ *   record is (dx, py0 - py1, z, z_prev) with dx = px0 - px1, and an invalid sample's record is (0, 0, NaN, NaN) (so a NaN z
+ *   also counts invalid).  Equirectangular: dx goes the short way round the seam, hw = (float)W * 0.5f,
+ *   dx = dx > hw ? dx - (float)W : (dx < -hw ? dx + (float)W : dx).
  * motion[4p + k] = (((+0 + r_a[k]) + r_b[k]) + ...) / (float)n over the n valid samples of the pixel in ascending sample
  * order; a pixel with n = 0, or outside the tile grid, is (0, 0, +inf, +inf), which never matches a history tap.
  * Both projections are the same function, so a static camera and a static scene give dx = dy = +0 and z_prev == z exactly
@@ -545,6 +568,19 @@ int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoi
                                                const RaynMomentPlanes* moments, const float* var_scale, float sigma_albedo,
                                                const float* albedo, int32_t width, int32_t height, const RaynFilmPlanes* in,
                                                const RaynFilmPlanes* out);
+/* The general form of the four entry points above on a film that is periodic in x (an equirectangular panorama, whose column 0
+ * and column W-1 are neighbours).  Which guides apply:
+ *   albedo == NULL: no albedo term (else sigma_albedo as in rayn_b200_film_denoise_albedo);
+ *   sigma_luminance == +inf: no variance term, and moments and var_scale are not read (rayn_b200_film_denoise or _albedo);
+ *   otherwise the variance term, with var_scale == NULL rayn_b200_film_denoise_variance, else _variance_scaled.
+ * The statement is the matching entry point's, except that every tap column, of the 5x5 filter and of the 3x3 variance
+ * prefilter, is taken floored-mod W: qx = ((x + dx) mod W + W) mod W in int.  Rows still skip taps outside the image: the poles
+ * do not wrap.  Every other rule (sigmas, skips, aliasing, spaces, asynchrony, errors) is the matching entry point's;
+ * sigma_luminance must be > 0.  Identities (tested): the result is the middle copy of the non-wrapped filter of the film tiled
+ * side by side often enough that no tap reaches an outer edge, bit for bit, and it commutes with rolling the film in x.    */
+int32_t rayn_b200_film_denoise_wrap(RaynContext* ctx, const RaynDenoiseDesc* desc, float sigma_luminance, int32_t spp,
+                                    const RaynMomentPlanes* moments, const float* var_scale, float sigma_albedo, const float* albedo,
+                                    int32_t width, int32_t height, const RaynFilmPlanes* in, const RaynFilmPlanes* out);
 
 /* ---- temporal accumulation of a frame sequence (the temporal half of SVGF, Schied et al. 2017; PAPERS.md) ---------------
  * A RaynTemporal holds the reprojectable history of one W x H film: per pixel colour 3, background 3, the 2 moments,
@@ -591,6 +627,13 @@ void rayn_b200_temporal_destroy(RaynTemporal* t);
 int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* desc, const RaynFilmPlanes* in,
                                 const RaynMomentPlanes* moments, const float* motion, const RaynFilmPlanes* out,
                                 const RaynMomentPlanes* out_moments, float* var_scale);
+/* rayn_b200_temporal_push on a film that is periodic in x (an equirectangular panorama): the same arguments and statement,
+ * except for the column test of a tap.  With the tap column qxf = x0 + (float)i (float, as above), the tap is inside in x if
+ * fabsf(qxf) <= 0x1p24f (false for NaN); then, in int, qx = ((int)qxf % W + W) % W is its history column.  So a non-finite dx
+ * takes no history, a huge one (|qxf| > 2^24) none either, and no index leaves the image.  Rows keep the in-image test.     */
+int32_t rayn_b200_temporal_push_wrap(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* desc, const RaynFilmPlanes* in,
+                                     const RaynMomentPlanes* moments, const float* motion, const RaynFilmPlanes* out,
+                                     const RaynMomentPlanes* out_moments, float* var_scale);
 
 /* ---- progressive / adaptive rendering: a device film accumulator refined in sample rounds -----------------------
  * Per-tile stopping rule after Dammertz, Hanika, Keller, Lensch (WSCG 2009; PAPERS.md): a tile's error compares the

@@ -9,7 +9,7 @@ Package layout (only what the hot path needs):
   dist.py    tile sharding across GPUs + NCCL film gather
   build.py   in-tree nvcc build of librayn_b200.so
 """
-from .scene import (BlackmanHarrisFilter, BoxFold, CameraStore, Dielectric, Emissive, HitableStore, Lambertian, Linear,  # noqa: F401
+from .scene import (BlackmanHarrisFilter, BoxFold, CameraStore, Dielectric, Emissive, EquirectangularCamera, HitableStore, Lambertian, Linear,  # noqa: F401
                     MandelBox, Mandelbulb, MaterialStore, OrbitTrapAlbedo, OrthographicCamera, PathTracingIntegrator, PinholeCamera,
                     RenderConsts, Sky, Sphere, SphereFold, SphereLight, Srgb, ThinLensCamera, TracedSDF, Vec3,
                     VolumeParams, World)

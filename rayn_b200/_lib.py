@@ -34,7 +34,7 @@ COMM_ID_BYTES = 128
 
 HITABLE_SPHERE, HITABLE_MANDELBOX, HITABLE_MANDELBULB = 0, 1, 2
 MATERIAL_LAMBERTIAN, MATERIAL_DIELECTRIC, MATERIAL_SKY, MATERIAL_EMISSIVE = 0, 1, 2, 3
-CAMERA_PINHOLE, CAMERA_THINLENS, CAMERA_ORTHOGRAPHIC = 0, 1, 2
+CAMERA_PINHOLE, CAMERA_THINLENS, CAMERA_ORTHOGRAPHIC, CAMERA_EQUIRECTANGULAR = 0, 1, 2, 3
 MEM_HOST, MEM_DEVICE = 0, 1
 POST_COLOR_PLUS_BACKGROUND, POST_COLOR_ALPHA, POST_COLOR_ONLY, POST_BACKGROUND, POST_WORLD_NORMAL, POST_ALPHA = range(6)
 POST_BYTES = (3, 4, 3, 3, 3, 1)
@@ -172,6 +172,10 @@ SYMBOLS = {
     "rayn_b200_render_motion_prev": (i32, [C.c_void_p, C.POINTER(RaynFrameDesc), f32, C.POINTER(RaynSceneDesc), C.c_void_p, C.c_void_p, i32]),
     "rayn_b200_film_denoise_variance_scaled": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), C.c_void_p, f32,
                                                      C.c_void_p, i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_film_denoise_wrap": (i32, [C.c_void_p, C.POINTER(RaynDenoiseDesc), f32, i32, C.POINTER(RaynMomentPlanes), C.c_void_p, f32, C.c_void_p,
+                                          i32, i32, C.POINTER(RaynFilmPlanes), C.POINTER(RaynFilmPlanes)]),
+    "rayn_b200_temporal_push_wrap": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynTemporalDesc), C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes),
+                                           C.c_void_p, C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes), C.c_void_p]),
     "rayn_b200_temporal_create": (i32, [C.c_void_p, i32, i32, C.POINTER(C.c_void_p)]),
     "rayn_b200_temporal_destroy": (None, [C.c_void_p]),
     "rayn_b200_temporal_push": (i32, [C.c_void_p, C.c_void_p, C.POINTER(RaynTemporalDesc), C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes),

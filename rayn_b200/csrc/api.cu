@@ -463,7 +463,7 @@ static int32_t validate_scene(RaynContext* ctx, const RaynSceneDesc* s) {
   for (int i = 0; i < s->n_materials; ++i)
     if (s->materials[i].kind < 0 || s->materials[i].kind > RAYN_MATERIAL_EMISSIVE)
       return fail(ctx, RAYN_ERR_INVALID_ARG, "material %d: bad kind %d", i, s->materials[i].kind);
-  if (s->camera.kind < 0 || s->camera.kind > RAYN_CAMERA_ORTHOGRAPHIC) return fail(ctx, RAYN_ERR_INVALID_ARG, "bad camera kind");
+  if (s->camera.kind < 0 || s->camera.kind > RAYN_CAMERA_EQUIRECTANGULAR) return fail(ctx, RAYN_ERR_INVALID_ARG, "bad camera kind");
   if (s->consts.max_marches < 1 || s->consts.max_vis_marches < 1) return fail(ctx, RAYN_ERR_INVALID_ARG, "march limits must be >= 1");
   return RAYN_OK;
 }
@@ -1619,10 +1619,10 @@ static bool denoise_factor(float sigma, float* f) {
 // mom != NULL (rayn_b200_film_denoise_variance with a finite sigma_luminance sl): the moment planes in in->space, 2 more
 // floats per pixel of staging when that is host memory; the variance travels in the .w lane of the ping-pong planes.
 // scale != NULL (rayn_b200_film_denoise_variance_scaled, with mom): the per-pixel variance scale in in->space, 1 more float per
-// pixel of staging when that is host memory.
+// pixel of staging when that is host memory.  wrap (rayn_b200_film_denoise_wrap): the film is periodic in x.
 static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W, int H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
                                float ic0, float in_, float ia, float* scratch, const float* albedo, float il, const RaynMomentPlanes* mom, float sl,
-                               int spp, const float* scale) {
+                               int spp, const float* scale, bool wrap) {
   cudaStream_t st = ctx->stream;
   const size_t npx = (size_t)W * H;
   const unsigned blocks1d = (unsigned)((npx + 255) / 256);
@@ -1678,13 +1678,13 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
       float4* dst4 = ping[(i + 1) & 1];
       const bool last = i == d->iterations - 1;
       if (albedo && mom)
-        denoise_level<true, true>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, sl);
+        denoise_level<true, true>(st, wrap, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, sl);
       else if (albedo)
-        denoise_level<true, false>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, 0.0f);
+        denoise_level<true, false>(st, wrap, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, alb, il, 0.0f);
       else if (mom)
-        denoise_level<false, true>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, sl);
+        denoise_level<false, true>(st, wrap, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, sl);
       else
-        denoise_level<false, false>(st, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, 0.0f);
+        denoise_level<false, false>(st, wrap, last, W, H, 1 << i, ic, in_, ia, guide, src, dst4, dst3, nullptr, 0.0f, 0.0f);
     }
     CU(cudaGetLastError());
     if (out->space == RAYN_MEM_HOST) CU(cudaMemcpyAsync(dst_user, dst3, npx * 12, cudaMemcpyDeviceToHost, st));
@@ -1694,10 +1694,10 @@ static int32_t denoise_enqueue(RaynContext* ctx, const RaynDenoiseDesc* d, int W
 
 // rayn_b200_film_denoise and, with an albedo plane (albedo != NULL), rayn_b200_film_denoise_albedo; with moment planes
 // (mom != NULL) and a finite sigma_luminance sl, rayn_b200_film_denoise_variance, and with a variance scale too (scale != NULL),
-// rayn_b200_film_denoise_variance_scaled
+// rayn_b200_film_denoise_variance_scaled; each of them periodic in x with wrap (rayn_b200_film_denoise_wrap)
 static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t W, int32_t H, const RaynFilmPlanes* in, const RaynFilmPlanes* out,
                             const float* albedo, float il, const RaynMomentPlanes* mom = nullptr, float sl = 0.0f, int spp = 0,
-                            const float* scale = nullptr) {
+                            const float* scale = nullptr, bool wrap = false) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!d || !in || !out || W <= 0 || H <= 0) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: bad argument");
   if (d->iterations < 1 || d->iterations > 8) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise: iterations %d not in [1,8]", d->iterations);
@@ -1721,7 +1721,7 @@ static int32_t film_denoise(RaynContext* ctx, const RaynDenoiseDesc* d, int32_t 
   float* scratch = nullptr;
   // stream-ordered and released below: nothing persists between calls (render-pass sizing reads cudaMemGetInfo)
   CU(cudaMallocAsync((void**)&scratch, nfloat * sizeof(float), st));
-  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il, mom, sl, spp, mom ? scale : nullptr);
+  const int32_t rc = denoise_enqueue(ctx, d, W, H, in, out, ic0, in_, ia, scratch, albedo, il, mom, sl, spp, mom ? scale : nullptr, wrap);
   const cudaError_t ef = cudaFreeAsync(scratch, st);
   if (rc) return rc;
   CU(ef);
@@ -1746,10 +1746,10 @@ int32_t rayn_b200_film_denoise_albedo(RaynContext* ctx, const RaynDenoiseDesc* d
   return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il);
 }
 
-// rayn_b200_film_denoise_variance (scale NULL) and rayn_b200_film_denoise_variance_scaled
+// rayn_b200_film_denoise_variance (scale NULL) and rayn_b200_film_denoise_variance_scaled, periodic in x with wrap
 static int32_t film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
                                      const float* scale, float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
-                                     const RaynFilmPlanes* out) {
+                                     const RaynFilmPlanes* out, bool wrap = false) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!moments || !in) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance: moments/in is NULL");
   if ((in->color && !moments->color_lum2) || (in->background && !moments->background_lum2))
@@ -1763,7 +1763,7 @@ static int32_t film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d,
                 sigma_albedo);
   // +inf: the term is not added (inf * sqrt(0) would be NaN), and the call is film_denoise / film_denoise_albedo
   const bool var = !isinf(sigma_luminance);
-  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, var ? moments : nullptr, sigma_luminance, spp, scale);
+  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, var ? moments : nullptr, sigma_luminance, spp, scale, wrap);
 }
 
 int32_t rayn_b200_film_denoise_variance(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
@@ -1778,6 +1778,20 @@ int32_t rayn_b200_film_denoise_variance_scaled(RaynContext* ctx, const RaynDenoi
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!var_scale) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_variance_scaled: var_scale is NULL");
   return film_denoise_variance(ctx, d, sigma_luminance, spp, moments, var_scale, sigma_albedo, albedo, W, H, in, out);
+}
+
+int32_t rayn_b200_film_denoise_wrap(RaynContext* ctx, const RaynDenoiseDesc* d, float sigma_luminance, int32_t spp, const RaynMomentPlanes* moments,
+                                    const float* var_scale, float sigma_albedo, const float* albedo, int32_t W, int32_t H, const RaynFilmPlanes* in,
+                                    const RaynFilmPlanes* out) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!(sigma_luminance > 0.0f)) return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_wrap: sigma_luminance %g must be > 0 (+inf disables the term)", sigma_luminance);
+  if (!isinf(sigma_luminance)) return film_denoise_variance(ctx, d, sigma_luminance, spp, moments, var_scale, sigma_albedo, albedo, W, H, in, out, true);
+  // no variance term: rayn_b200_film_denoise, or rayn_b200_film_denoise_albedo's rules for the albedo guide
+  float il = 0.0f;
+  if (albedo && !denoise_factor(sigma_albedo, &il))
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "film_denoise_wrap: sigma_albedo %g must be > 0 (+inf disables the term) and give a finite 1/sigma^2",
+                sigma_albedo);
+  return film_denoise(ctx, d, W, H, in, out, il == 0.0f ? nullptr : albedo, il, nullptr, 0.0f, 0, nullptr, true);
 }
 
 int32_t rayn_b200_device_frame_inputs(RaynContext* ctx, int32_t W, int32_t H, int32_t spp, int32_t sets_1d, int32_t sets_2d, uint64_t offset,
@@ -1988,8 +2002,9 @@ void rayn_b200_temporal_destroy(RaynTemporal* t) {
   delete t;
 }
 
-int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* d, const RaynFilmPlanes* in, const RaynMomentPlanes* mom,
-                                const float* motion, const RaynFilmPlanes* out, const RaynMomentPlanes* omom, float* scale) {
+// rayn_b200_temporal_push, and with wrap rayn_b200_temporal_push_wrap (history tap columns floored-mod W)
+static int32_t temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* d, const RaynFilmPlanes* in, const RaynMomentPlanes* mom,
+                             const float* motion, const RaynFilmPlanes* out, const RaynMomentPlanes* omom, float* scale, bool wrap) {
   if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
   if (!t || !d || !in || !mom || !motion || !out || !omom || !scale) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: NULL argument");
   if (t->device != ctx->device) return fail(ctx, RAYN_ERR_INVALID_ARG, "temporal_push: the history lives on device %d, the context on %d", t->device, ctx->device);
@@ -2026,7 +2041,11 @@ int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTem
       CU(e);
     }
   }
-  k_temporal<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(t->W, t->H, *d, t->hist[t->cur], t->hist[t->cur ^ 1], io);
+  const unsigned blocks = (unsigned)((npx + 255) / 256);
+  if (wrap)
+    k_temporal<true><<<blocks, 256, 0, st>>>(t->W, t->H, *d, t->hist[t->cur], t->hist[t->cur ^ 1], io);
+  else
+    k_temporal<false><<<blocks, 256, 0, st>>>(t->W, t->H, *d, t->hist[t->cur], t->hist[t->cur ^ 1], io);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) t->cur ^= 1;
   if (sp == RAYN_MEM_HOST) {
@@ -2040,6 +2059,17 @@ int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTem
   }
   CU(e);
   return RAYN_OK;
+}
+
+int32_t rayn_b200_temporal_push(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* d, const RaynFilmPlanes* in, const RaynMomentPlanes* mom,
+                                const float* motion, const RaynFilmPlanes* out, const RaynMomentPlanes* omom, float* scale) {
+  return temporal_push(ctx, t, d, in, mom, motion, out, omom, scale, false);
+}
+
+int32_t rayn_b200_temporal_push_wrap(RaynContext* ctx, RaynTemporal* t, const RaynTemporalDesc* d, const RaynFilmPlanes* in,
+                                     const RaynMomentPlanes* mom, const float* motion, const RaynFilmPlanes* out, const RaynMomentPlanes* omom,
+                                     float* scale) {
+  return temporal_push(ctx, t, d, in, mom, motion, out, omom, scale, true);
 }
 
 // ---- known-answer entry points ----------------------------------------------------------------------

@@ -29,6 +29,13 @@ __device__ __forceinline__ bool dn_finite3(const float4 c) { return isfinite(c.x
 // is rounded on its own as the header states.
 __host__ __device__ __forceinline__ float dn_lum(float r, float g, float b) { return (0.2126f * r + 0.7152f * g) + 0.0722f * b; }
 
+// floored q mod W, in [0, W): the column of tap q on a film that is periodic in x.  Only the taps near the seam divide.
+__device__ __forceinline__ int dn_wrap(int q, int W) {
+  if ((unsigned)q < (unsigned)W) return q;
+  q %= W;
+  return q < 0 ? q + W : q;
+}
+
 // planes -> float4 (r, g, b, 0) / (nx, ny, nz, a)
 __global__ void __launch_bounds__(256) k_denoise_pack(long long npx, const float* __restrict__ c3, float4* __restrict__ out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -63,7 +70,8 @@ __global__ void __launch_bounds__(256) k_denoise_pack_var(long long npx, const f
 // il_p = 1 / (sl * sqrt(g_p) + 1e-10), g_p the 3x3 prefilter of v, and the output's .w is the filtered variance
 // (sum (w*w) v_q) / (sw*sw).  The prefilter is fused here: its 9 taps are neighbours of p that the 5x5 loop's first level
 // reads too, so they are L1 hits, and no extra plane or launch is needed.  The kVar = false instances never read `sl`.
-template <bool kOut3, bool kAlb = false, bool kVar = false>
+// kWrap (rayn_b200_film_denoise_wrap): the film is periodic in x, every tap column is taken floored-mod W; rows still skip.
+template <bool kOut3, bool kAlb = false, bool kVar = false, bool kWrap = false>
 __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, float ic, float in_, float ia, const float4* __restrict__ guide,
                                                        const float4* __restrict__ src, float4* __restrict__ dst4, float* __restrict__ dst3,
                                                        const float4* __restrict__ alb = nullptr, float il = 0.0f, float sl = 0.0f) {
@@ -88,8 +96,12 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
         if (qy < 0 || qy >= H) continue;
 #pragma unroll
         for (int dx = -1; dx <= 1; ++dx) {
-          const int qx = x + dx;
-          if (qx < 0 || qx >= W) continue;
+          int qx = x + dx;
+          if (kWrap) {
+            qx = dn_wrap(qx, W);
+          } else if (qx < 0 || qx >= W) {
+            continue;
+          }
           const float4 cq = src[(size_t)qy * W + qx];
           if (!dn_finite3(cq)) continue;
           const float kk = k3[dy + 1] * k3[dx + 1];
@@ -107,8 +119,12 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
       const float4* grow = guide + (size_t)qy * W;
 #pragma unroll
       for (int dx = -2; dx <= 2; ++dx) {
-        const int qx = x + step * dx;
-        if (qx < 0 || qx >= W) continue;
+        int qx = x + step * dx;
+        if (kWrap) {
+          qx = dn_wrap(qx, W);
+        } else if (qx < 0 || qx >= W) {
+          continue;
+        }
         const float4 cq = srow[qx];
         if (!dn_finite3(cq)) continue;
         const float4 gq = grow[qx];
@@ -161,15 +177,23 @@ __global__ void __launch_bounds__(256) k_denoise_level(int W, int H, int step, f
   }
 }
 
-// One level of the filter: the k_denoise_level instance of (last level, albedo guide, variance guide)
-template <bool kAlb, bool kVar>
+// One level of the filter: the k_denoise_level instance of (last level, albedo guide, variance guide, periodic in x)
+template <bool kAlb, bool kVar, bool kWrap>
 inline void denoise_level(cudaStream_t st, bool last, int W, int H, int step, float ic, float in_, float ia, const float4* guide, const float4* src,
                           float4* dst4, float* dst3, const float4* alb, float il, float sl) {
   const dim3 blk(32, 8), grid((unsigned)((W + 31) / 32), (unsigned)((H + 7) / 8));
   if (last)
-    k_denoise_level<true, kAlb, kVar><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, nullptr, dst3, alb, il, sl);
+    k_denoise_level<true, kAlb, kVar, kWrap><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, nullptr, dst3, alb, il, sl);
   else
-    k_denoise_level<false, kAlb, kVar><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, dst4, nullptr, alb, il, sl);
+    k_denoise_level<false, kAlb, kVar, kWrap><<<grid, blk, 0, st>>>(W, H, step, ic, in_, ia, guide, src, dst4, nullptr, alb, il, sl);
+}
+template <bool kAlb, bool kVar>
+inline void denoise_level(cudaStream_t st, bool wrap, bool last, int W, int H, int step, float ic, float in_, float ia, const float4* guide,
+                          const float4* src, float4* dst4, float* dst3, const float4* alb, float il, float sl) {
+  if (wrap)
+    denoise_level<kAlb, kVar, true>(st, last, W, H, step, ic, in_, ia, guide, src, dst4, dst3, alb, il, sl);
+  else
+    denoise_level<kAlb, kVar, false>(st, last, W, H, step, ic, in_, ia, guide, src, dst4, dst3, alb, il, sl);
 }
 
 }  // namespace rt

@@ -610,6 +610,15 @@ RT_D void camera_ray(const RaynCamera& c, float u, float v, float ls0, float ls1
     f3 o2 = origin + offset;
     *ro = o2;
     *rd = normalized(lower_left + horiz + verti - o2);
+  } else if (c.kind == RAYN_CAMERA_EQUIRECTANGULAR) {  // EXTENSION, no reference counterpart (include/rayn_b200.h)
+    f3 bw = normalized(origin - at);
+    f3 bu = normalized(cross(up, bw));
+    f3 bv = cross(bw, bu);
+    float sp, cp, st, ct;
+    dm::sincos((u - 0.5f) * RT_TWO_PI, &sp, &cp);
+    dm::sincos((v - 0.5f) * RT_PI, &st, &ct);
+    *ro = origin;
+    *rd = normalized(bu * (ct * sp) + bv * st - bw * (ct * cp));
   } else {  // orthographic :249-280
     f3 bw = normalized(at - origin);
     f3 bu = normalized(cross(bw, up));

@@ -37,6 +37,14 @@ RT_D void camera_project(const RaynCamera& c, int W, int H, f3 X, float time, fl
     *z = dot(r, bw);
     *px = ((dot(r, bu) + hx) / c.full_size[0]) * (float)W;
     *py = ((dot(r, bv) + hy) / c.full_size[1]) * (float)H;
+  } else if (c.kind == RAYN_CAMERA_EQUIRECTANGULAR) {  // z is the distance; px, py invert the angles of camera_ray
+    const f3 bw = normalized(origin - at);
+    const f3 bu = normalized(cross(up, bw));
+    const f3 bv = cross(bw, bu);
+    const float xr = dot(r, bu), yr = dot(r, bv), zr = -dot(r, bw);
+    *z = mag(r);
+    *px = (dm::atan2(xr, zr) / RT_TWO_PI + 0.5f) * (float)W;
+    *py = (dm::atan2(yr, sqrtf(xr * xr + zr * zr)) / RT_PI + 0.5f) * (float)H;
   } else {
     const f3 bw = normalized(origin - at);
     const f3 bu = normalized(cross(up, bw));
@@ -90,7 +98,14 @@ __global__ void __launch_bounds__(256) k_first_hit_paths(const __grid_constant__
       float px1, py1, z1, px0, py0, z0;
       camera_project(sc.cam, fr.W, fr.H, P, tau, &px1, &py1, &z1);
       camera_project(kPrev ? pv->cam : sc.cam, fr.W, fr.H, Pp, tau - frame_dt, &px0, &py0, &z0);
-      if (sc.cam.kind == RAYN_CAMERA_ORTHOGRAPHIC || (z1 > 0.0f && z0 > 0.0f)) rec = make_float4(px0 - px1, py0 - py1, z1, z0);
+      if (sc.cam.kind == RAYN_CAMERA_ORTHOGRAPHIC || (z1 > 0.0f && z0 > 0.0f)) {
+        float dx = px0 - px1;
+        if (sc.cam.kind == RAYN_CAMERA_EQUIRECTANGULAR) {  // the short way round the seam
+          const float hw = (float)fr.W * 0.5f;
+          dx = dx > hw ? dx - (float)fr.W : (dx < -hw ? dx + (float)fr.W : dx);
+        }
+        rec = make_float4(dx, py0 - py1, z1, z0);
+      }
     }
     if constexpr (kAlb) a = first_hit_albedo(sc, h, P);
   }

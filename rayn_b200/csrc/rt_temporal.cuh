@@ -16,6 +16,8 @@ struct TemporalIo {
   float *oc, *ob, *omc, *omb, *scale;          // outputs (oc / ob may alias c / b)
 };
 
+// kWrap (rayn_b200_temporal_push_wrap): the film is periodic in x, history tap columns are taken floored-mod W
+template <bool kWrap>
 __global__ void __launch_bounds__(256) k_temporal(int W, int H, RaynTemporalDesc d, const float* __restrict__ hin, float* __restrict__ hout,
                                                   TemporalIo io) {
   const long long npx = (long long)W * H;
@@ -44,9 +46,18 @@ __global__ void __launch_bounds__(256) k_temporal(int W, int H, RaynTemporalDesc
       for (int i = 0; i < 2; ++i) {
         const float w = (i ? ax : 1.0f - ax) * (j ? ay : 1.0f - ay);
         const float qxf = x0 + (float)i, qyf = y0 + (float)j;
-        // NaN motion fails every comparison: no tap
-        if (!(w != 0.0f) || !(qxf >= 0.0f && qxf <= (float)(W - 1) && qyf >= 0.0f && qyf <= (float)(H - 1))) continue;
-        const size_t q = (size_t)qyf * W + (size_t)qxf;
+        size_t q;
+        if constexpr (kWrap) {
+          // the column test of rayn_b200_temporal_push_wrap: |qxf| <= 2^24 (false for NaN) makes (int)qxf exact and in range
+          if (!(w != 0.0f) || !(fabsf(qxf) <= 0x1p24f && qyf >= 0.0f && qyf <= (float)(H - 1))) continue;
+          int qx = (int)qxf % W;
+          if (qx < 0) qx += W;
+          q = (size_t)qyf * W + (size_t)qx;
+        } else {
+          // NaN motion fails every comparison: no tap
+          if (!(w != 0.0f) || !(qxf >= 0.0f && qxf <= (float)(W - 1) && qyf >= 0.0f && qyf <= (float)(H - 1))) continue;
+          q = (size_t)qyf * W + (size_t)qxf;
+        }
         if (!(hin[TH_LEN * npx + q] > 0.0f)) continue;
         const float c0 = hin[TH_C * npx + q], c1 = hin[(TH_C + 1) * npx + q], c2 = hin[(TH_C + 2) * npx + q];
         const float b0 = hin[TH_B * npx + q], b1 = hin[(TH_B + 1) * npx + q], b2 = hin[(TH_B + 2) * npx + q];

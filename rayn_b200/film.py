@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib as L
-from .scene import BlackmanHarrisFilter, PathTracingIntegrator
+from .scene import BlackmanHarrisFilter, EquirectangularCamera, PathTracingIntegrator
 
 CHANNELS = ("color", "alpha", "background", "normal")  # ChannelKind, film.rs:103-120
 # a Film may also hold the first-hit albedo plane (Renderer.render_albedo) and the luminance second moments of its colour
@@ -121,6 +121,20 @@ ADAPTIVE_MAX_ROUNDS = 32
 
 def adaptive_desc(min_rounds=2, max_rounds=ADAPTIVE_MAX_ROUNDS, threshold=ADAPTIVE_THRESHOLD):
     return L.RaynAdaptiveDesc(int(min_rounds), int(max_rounds), float(threshold))
+
+
+def check_panorama_width(world, camera, width, tile_size):
+    """Raises ValueError if the camera (a handle into world.cameras) is an EquirectangularCamera whose film width the tile grid
+    does not cover: the grid of film.rs:399-404
+    drops the last partial tile when 0 < width % tile_w < tile_w / 2, which would leave a black strip at the seam.  Returns
+    whether the camera is a panorama."""
+    if not isinstance(world.cameras.get(camera), EquirectangularCamera):
+        return False
+    r = width % tile_size[0]
+    if 0 < r and 2 * r < tile_size[0]:
+        raise ValueError(f"a panorama {width} pixels wide leaves its last {r} columns out of the {tile_size[0]}-wide tile grid (black at "
+                         f"the seam): use a width whose remainder modulo the tile width is 0 or at least half a tile")
+    return True
 
 
 def tile_grid(width, height, tile_w, tile_h):
@@ -292,10 +306,11 @@ class Renderer:
     def temporal_create(self, width, height):
         return Temporal(self, width, height)
 
-    def temporal_push(self, t, planes, moments, motion, alpha_min, sigma_depth, normal_cos, reset=False):
+    def temporal_push(self, t, planes, moments, motion, alpha_min, sigma_depth, normal_cos, reset=False, wrap=False):
         """Blends one frame into the history t (include/rayn_b200.h: rayn_b200_temporal_push).  planes: numpy "color",
         "background" and "normal"; moments float32 [H, W, 2]; motion float32 [H, W, 4] (render_motion's).  Returns
-        (planes with new "color" / "background", moments [H, W, 2], var_scale [H, W]) as float32 arrays."""
+        (planes with new "color" / "background", moments [H, W, 2], var_scale [H, W]) as float32 arrays.  wrap=True: the film is
+        periodic in x, a panorama's (rayn_b200_temporal_push_wrap)."""
         w, h = t.width, t.height
         flat = {k: np.ascontiguousarray(planes[k], np.float32).reshape(-1) for k in ("color", "background", "normal")}
         m = np.ascontiguousarray(np.asarray(moments, np.float32).reshape(h, w, 2).transpose(2, 0, 1)).reshape(2, -1)
@@ -307,7 +322,8 @@ class Renderer:
         mi = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
         mo = L.RaynMomentPlanes(om[0].ctypes.data, om[1].ctypes.data, L.MEM_HOST)
         d = L.RaynTemporalDesc(float(alpha_min), float(sigma_depth), float(normal_cos), 1 if reset else 0)
-        L.check(self._lib.rayn_b200_temporal_push(self._ctx, t.handle, C.byref(d), C.byref(pin), C.byref(mi), mv.ctypes.data, C.byref(pout),
+        push = self._lib.rayn_b200_temporal_push_wrap if wrap else self._lib.rayn_b200_temporal_push
+        L.check(push(self._ctx, t.handle, C.byref(d), C.byref(pin), C.byref(mi), mv.ctypes.data, C.byref(pout),
                                                   C.byref(mo), scale.ctypes.data), self._ctx)
         out = {"color": oc.reshape(np.shape(planes["color"])), "background": ob.reshape(np.shape(planes["background"]))}
         return out, np.ascontiguousarray(om.reshape(2, h, w).transpose(1, 2, 0)), scale.reshape(h, w)
@@ -322,7 +338,7 @@ class Renderer:
         return out
 
     def denoise(self, width, height, planes, iterations=5, sigma_color=None, sigma_normal=None, sigma_alpha=None, albedo=None,
-                sigma_albedo=None, moments=None, spp=None, sigma_luminance=None, var_scale=None):
+                sigma_albedo=None, moments=None, spp=None, sigma_luminance=None, var_scale=None, wrap=False):
         """Edge-avoiding a-trous filter of the color and background planes (include/rayn_b200.h: rayn_b200_film_denoise).
         numpy planes in ("normal" and "alpha" required, "color" / "background" optional); returns new arrays for the
         colour planes given, shaped like their inputs.  Sigmas default to DENOISE_DEFAULTS; +inf disables a term.
@@ -330,7 +346,8 @@ class Renderer:
         sigma_albedo, default DENOISE_ALBEDO_SIGMA.  moments (float32 [H, W, 2], render_host(moments=True)'s) with the film's
         spp: the variance-guided filter (rayn_b200_film_denoise_variance) with sigma_luminance, default
         DENOISE_LUMINANCE_SIGMA, and sigma_color defaulting to DENOISE_VARIANCE_SIGMA_COLOR; combinable with albedo.
-        var_scale (float32 [H, W], temporal_push's), with moments: rayn_b200_film_denoise_variance_scaled."""
+        var_scale (float32 [H, W], temporal_push's), with moments: rayn_b200_film_denoise_variance_scaled.  wrap=True: the same
+        filter on a film that is periodic in x, a panorama's (rayn_b200_film_denoise_wrap)."""
         for k in ("normal", "alpha"):
             if planes.get(k) is None:
                 raise ValueError(f"denoise needs the {k} guide plane")
@@ -347,7 +364,20 @@ class Renderer:
             sigma_color = DENOISE_VARIANCE_SIGMA_COLOR
         desc = denoise_desc(iterations, sigma_color, sigma_normal, sigma_alpha)
         sa = float(DENOISE_ALBEDO_SIGMA if sigma_albedo is None else sigma_albedo)
-        if moments is not None:
+        if var_scale is not None and moments is None:
+            raise ValueError("var_scale scales the variance of the moments: pass moments too")
+        if wrap:
+            m = mp = None
+            if moments is not None:
+                m = np.ascontiguousarray(np.asarray(moments, np.float32).reshape(height, width, 2).transpose(2, 0, 1)).reshape(2, -1)
+                mp = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
+            sl = float(DENOISE_LUMINANCE_SIGMA if sigma_luminance is None else sigma_luminance) if moments is not None else float("inf")
+            alb = None if albedo is None else np.ascontiguousarray(albedo, np.float32).reshape(-1)
+            vs = None if var_scale is None else np.ascontiguousarray(var_scale, np.float32).reshape(-1)
+            L.check(self._lib.rayn_b200_film_denoise_wrap(self._ctx, C.byref(desc), sl, 0 if spp is None else int(spp), None if mp is None else C.byref(mp),
+                                                          None if vs is None else vs.ctypes.data, sa, None if alb is None else alb.ctypes.data,
+                                                          width, height, C.byref(pin), C.byref(pout)), self._ctx)
+        elif moments is not None:
             m = np.ascontiguousarray(np.asarray(moments, np.float32).reshape(height, width, 2).transpose(2, 0, 1)).reshape(2, -1)
             mp = L.RaynMomentPlanes(m[0].ctypes.data, m[1].ctypes.data, L.MEM_HOST)
             sl = float(DENOISE_LUMINANCE_SIGMA if sigma_luminance is None else sigma_luminance)
@@ -360,8 +390,6 @@ class Renderer:
                 vs = np.ascontiguousarray(var_scale, np.float32).reshape(-1)
                 L.check(self._lib.rayn_b200_film_denoise_variance_scaled(self._ctx, C.byref(desc), sl, int(spp), C.byref(mp), vs.ctypes.data, sa,
                                                                          alb_p, width, height, C.byref(pin), C.byref(pout)), self._ctx)
-        elif var_scale is not None:
-            raise ValueError("var_scale scales the variance of the moments: pass moments too")
         elif albedo is None:
             L.check(self._lib.rayn_b200_film_denoise(self._ctx, C.byref(desc), width, height, C.byref(pin), C.byref(pout)), self._ctx)
         else:
@@ -510,9 +538,11 @@ class Film:
         self._device = device
         self.last_stats = None
         self.spp = None  # samples per pixel of the last render_frame_into (the "moments" channel's count)
+        self.panorama = False  # the last render used an EquirectangularCamera: the film is periodic in x, and denoise wraps
 
     def render_frame_into(self, world, camera, integrator, filt, tile_size, frame, time_range, samples):
         """Drop-in for film.rs:382-395.  time_range = (start, end)."""
+        panorama = check_panorama_width(world, camera, self.res[0], tile_size)
         if self._renderer is None:
             self._renderer = Renderer(self._device)
         w, h = self.res
@@ -527,6 +557,7 @@ class Film:
             elif k not in ("albedo", "motion"):  # "motion" is filled by render_sequence
                 self.channels[k] = planes[k].reshape((h, w, 3) if k != "alpha" else (h, w))
         self._render_albedo(integrator, filt, tile_size, frame, time_range, samples)
+        self.panorama = panorama
         self.progressive_epoch += 1  # film.rs:657
 
     def _render_albedo(self, integrator, filt, tile_size, frame, time_range, samples):
@@ -550,6 +581,7 @@ class Film:
             raise ValueError("render_adaptive does not fold luminance moments: use render_frame_into for a Film with \"moments\"")
         if "motion" in self.channel_kinds:
             raise ValueError("render_adaptive renders no motion plane: use render_sequence for a Film with \"motion\"")
+        panorama = check_panorama_width(world, camera, self.res[0], tile_size)
         import torch  # device buffers for the sample tables and the scramble plane
         if self._renderer is None:
             self._renderer = Renderer(self._device)
@@ -588,6 +620,7 @@ class Film:
         finally:
             acc.close()
         self._render_albedo(integrator, filt, tile_size, frame, time_range, samples_per_round * max_rounds)
+        self.panorama = panorama
         return rounds
 
     def _take_accum(self, r, acc):
@@ -612,12 +645,14 @@ class Film:
         A world with closure parameters (World.has_closures: a sphere on a curved path, an orbiting camera) is uploaded
         before every frame as its chord over that frame's time range, and every frame after the first measures its motion
         against the scene the previous frame was rendered with (Renderer.render_motion(prev=...)).  Any other world is
-        uploaded once and its motion is the uploaded scene run backwards."""
+        uploaded once and its motion is the uploaded scene run backwards.  With an EquirectangularCamera the push and the
+        denoise wrap round the seam (Renderer.temporal_push / denoise with wrap=True)."""
         if "moments" in self.channel_kinds:
             raise ValueError("render_sequence consumes the moments of every frame: create the Film without \"moments\"")
         for k in ("color", "background", "alpha", "normal"):
             if k not in self.channel_kinds:
                 raise ValueError(f"render_sequence needs the {k} channel")
+        panorama = check_panorama_width(world, camera, self.res[0], tile_size)
         t_kw = {k: float(TEMPORAL_DEFAULTS[k] if v is None else v)
                 for k, v in dict(alpha_min=alpha_min, sigma_depth=sigma_depth, normal_cos=normal_cos).items()}
         animated = world.has_closures(camera)
@@ -647,16 +682,17 @@ class Film:
                     motion, albedo = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, albedo=True, prev=p_desc)
                 else:
                     motion = r.render_motion(g_inputs, tile_size, integrator, time_range, frame_dt, prev=p_desc)
-                blend, moments, scale = r.temporal_push(hist, planes, planes["moments"], motion, reset=(n == 0), **t_kw)
+                blend, moments, scale = r.temporal_push(hist, planes, planes["moments"], motion, reset=(n == 0), wrap=panorama, **t_kw)
                 guides = {"color": blend["color"], "background": blend["background"], "alpha": planes["alpha"], "normal": planes["normal"]}
                 out = r.denoise(w, h, guides, iterations, albedo=None if albedo is None else albedo.reshape(-1), moments=moments,
-                                spp=inputs.spp, var_scale=scale)
+                                spp=inputs.spp, var_scale=scale, wrap=panorama)
                 self.channels = {"color": out["color"].reshape(h, w, 3), "background": out["background"].reshape(h, w, 3),
                                  "alpha": planes["alpha"].reshape(h, w), "normal": planes["normal"].reshape(h, w, 3)}
                 if albedo is not None:
                     self.channels["albedo"] = albedo
                 if "motion" in self.channel_kinds:
                     self.channels["motion"] = motion
+                self.panorama = panorama
                 self.progressive_epoch += 1
                 n += 1
                 if on_frame is not None:
@@ -706,7 +742,7 @@ class Film:
         variance if it has the moments channel (sigma_luminance, default DENOISE_LUMINANCE_SIGMA).  Call it after
         render_frame_into and before save_to.  The moments describe the unfiltered render, so the variance-guided filter
         removes the "moments" channel from self.channels (a later call filters without it; render_frame_into fills it
-        again)."""
+        again).  A panorama's film (self.panorama) is filtered across the seam (Renderer.denoise(wrap=True))."""
         for k in ("normal", "alpha"):
             if k not in self.channels:
                 raise ValueError(f"Film.denoise needs the {k} channel")
@@ -717,13 +753,14 @@ class Film:
             self.channels.update(self._renderer.denoise(w, h, {k: self.channels.get(k) for k in CHANNELS}, iterations, sigma_color,
                                                         sigma_normal, sigma_alpha, albedo=self.channels.get("albedo"),
                                                         sigma_albedo=sigma_albedo, moments=self.channels["moments"], spp=self.spp,
-                                                        sigma_luminance=sigma_luminance))
+                                                        sigma_luminance=sigma_luminance, wrap=self.panorama))
             del self.channels["moments"]  # M - lum(c)^2 of filtered colour is not the variance of anything
         elif "albedo" in self.channels:
             self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha,
-                                                        albedo=self.channels["albedo"], sigma_albedo=sigma_albedo))
+                                                        albedo=self.channels["albedo"], sigma_albedo=sigma_albedo, wrap=self.panorama))
         else:
-            self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha))
+            self.channels.update(self._renderer.denoise(w, h, self.channels, iterations, sigma_color, sigma_normal, sigma_alpha,
+                                                        wrap=self.panorama))
 
     def tonemapped_rgb8(self):
         """The display formula of save_to (film.rs:253-267): (color + background).saturated().gamma(2.2), y flipped."""

@@ -1,11 +1,14 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
 //   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] [--denoise L]
-//             [--denoise-albedo] [--denoise-variance] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out file.ppm] [--dump planes.bin]
+//             [--denoise-albedo] [--denoise-variance] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--panorama] [--out file.ppm] [--dump planes.bin]
 // --denoise-albedo (with --denoise) renders the first-hit albedo plane as rayn_b200.film.Film does and guides the filter with it.
 // --denoise-variance (with --denoise, not with --adaptive) renders the frame with its luminance moments and weights each
 // pixel's colour by its own variance, as rayn_b200.film.Film does with a "moments" channel; combinable with --denoise-albedo.
 // --orbit-trap colours the fractal of configs 2-5 by orbit trap: albedo (R0 G0 B0) at trap LO, (R1 G1 B1) at HI
 // (include/rayn_b200.h, RaynAlbedoTrap; tools/trap_range.py prints a range for config 3).
+// --panorama replaces the config's camera with a 360-degree equirectangular one at the same origin, at and up (include/rayn_b200.h,
+// RAYN_CAMERA_EQUIRECTANGULAR), as rayn_b200.EquirectangularCamera; --denoise then filters across the seam
+// (rayn_b200_film_denoise_wrap).  W must leave no partial tile narrower than half a tile (the reference tile grid drops it).
 // Renders one frame (frame 1, shutter 1/24 at 24 fps: main.rs:47-49,61-62), prints the reference's
 // "Done in {s} seconds." line (main.rs:79-82) and writes the display image with the formula of
 // Film::save_to (film.rs:253-267): (color + background).saturated().gamma_corrected(2.2), y flipped.
@@ -81,7 +84,7 @@ int main(int argc, char** argv) {
   int max_rounds = kAdaptiveMaxRounds;
   bool res_set = false, samples_set = false, bounces_set = false;
   const char *out = nullptr, *dump = nullptr, *dump_scene = nullptr;
-  bool orbit_trap = false;
+  bool orbit_trap = false, panorama = false;
   OrbitTrapAlbedo trap{0.0f, 1.0f, Srgb(0, 0, 0), Srgb(0, 0, 0)};
   for (int i = 1; i < argc; ++i) {
     if (!strcmp(argv[i], "--config") && i + 1 < argc) config = atoi(argv[++i]);
@@ -94,6 +97,7 @@ int main(int argc, char** argv) {
     else if (!strcmp(argv[i], "--denoise") && i + 1 < argc) denoise = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--denoise-albedo")) denoise_albedo = true;
     else if (!strcmp(argv[i], "--denoise-variance")) denoise_variance = true;
+    else if (!strcmp(argv[i], "--panorama")) panorama = true;
     else if (!strcmp(argv[i], "--adaptive") && i + 1 < argc) adaptive = true, threshold = (float)atof(argv[++i]);
     else if (!strcmp(argv[i], "--rounds") && i + 1 < argc) max_rounds = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--orbit-trap") && i + 8 < argc) {
@@ -103,7 +107,8 @@ int main(int argc, char** argv) {
       orbit_trap = true;
     } else {
       fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] "
-                      "[--denoise L [--denoise-albedo] [--denoise-variance]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--out f.ppm] [--dump f.bin]\n");
+                      "[--denoise L [--denoise-albedo] [--denoise-variance]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--panorama] [--out f.ppm] "
+                      "[--dump f.bin]\n");
       return 2;
     }
   }
@@ -119,11 +124,20 @@ int main(int argc, char** argv) {
   if (!res_set) W = cfg_res[config][0], H = cfg_res[config][1];
   if (!samples_set) samples = cfg_samples[config];
   if (!bounces_set) bounces = cfg_bounces[config];
+  if (panorama && panorama_width_uncovered(W, 16)) {
+    fprintf(stderr, "--panorama: the 16-wide tile grid leaves the last %d of %d columns out (black at the seam); pick another width\n", W % 16, W);
+    return 2;
+  }
   try {
     World world;
-    const CameraHandle camera = config == 1 ? setup_single_sphere(world, (float)W, (float)H)
-                                            : setup(world, (float)W, (float)H, config == 4, config == 3 ? 0 : 1, config == 4,
-                                                    orbit_trap ? &trap : nullptr);
+    CameraHandle camera = config == 1 ? setup_single_sphere(world, (float)W, (float)H)
+                                      : setup(world, (float)W, (float)H, config == 4, config == 3 ? 0 : 1, config == 4,
+                                              orbit_trap ? &trap : nullptr);
+    if (panorama) {
+      const RaynCamera& c = world.cameras.get(camera);
+      camera = world.cameras.add_camera(EquirectangularCamera((float)H, Vec3(c.origin[0], c.origin[1], c.origin[2]), Vec3(c.at[0], c.at[1], c.at[2]),
+                                                              Vec3(c.up[0], c.up[1], c.up[2])));
+    }
     if (dump_scene) {  // flattened World as raw PODs (no GPU needed): hitables | materials | lights | camera | volume
       FILE* f = fopen(dump_scene, "wb");
       if (!f) { perror(dump_scene); return 1; }
@@ -161,7 +175,10 @@ int main(int argc, char** argv) {
     if (denoise_albedo)
       film.render_albedo(world, camera, integrator, filter, 16, 16, frame, frame_start, frame_end,
                          std::min(adaptive ? samples * max_rounds : samples, kAlbedoSamples));
-    if (denoise_variance) {
+    if (denoise && panorama) {
+      film.denoise_wrap(denoise, denoise_variance ? kDenoiseVarianceSigmaColor : kDenoiseSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha,
+                        denoise_variance ? kDenoiseLuminanceSigma : INFINITY, denoise_albedo, kDenoiseAlbedoSigma);
+    } else if (denoise_variance) {
       film.denoise_variance(denoise, kDenoiseVarianceSigmaColor, kDenoiseSigmaNormal, kDenoiseSigmaAlpha, kDenoiseLuminanceSigma, denoise_albedo,
                             kDenoiseAlbedoSigma);
     } else if (denoise_albedo) {

@@ -218,6 +218,22 @@ struct OrthographicCamera : Camera {  // camera.rs:227-241
     origin.velocity.store(pod.origin_velocity), at.velocity.store(pod.at_velocity), up.velocity.store(pod.up_velocity);
   }
 };
+// A 360-degree equirectangular panorama (include/rayn_b200.h, RAYN_CAMERA_EQUIRECTANGULAR): an EXTENSION with no reference
+// counterpart.  half_pixel_size is the angular half pixel, as rayn_b200/scene.py EquirectangularCamera computes it.
+struct EquirectangularCamera : Camera {
+  EquirectangularCamera(float ry, Seq3 origin, Seq3 at, Seq3 up) {
+    pod.kind = RAYN_CAMERA_EQUIRECTANGULAR;
+    pod.half_pixel_size = (3.14159265358979323846f / ry) / 2.0f;
+    origin.base.store(pod.origin), at.base.store(pod.at), up.base.store(pod.up);
+    origin.velocity.store(pod.origin_velocity), at.velocity.store(pod.at_velocity), up.velocity.store(pod.up_velocity);
+  }
+};
+// true if the tile grid of film.rs:399-404 leaves the last columns of a film `width` pixels wide out (0 < width % tile_w <
+// tile_w / 2): a panorama would show a black strip at the seam
+inline bool panorama_width_uncovered(int width, int tile_w) {
+  const int r = width % tile_w;
+  return 0 < r && 2 * r < tile_w;
+}
 struct CameraStore {  // camera.rs:24-40
   std::vector<RaynCamera> items;
   CameraHandle add_camera(const Camera& c) {
@@ -376,6 +392,21 @@ class Film {
     check(rayn_b200_film_denoise_variance(ctx_, &d, sigma_luminance, spp_, &m, sigma_albedo, with_albedo ? albedo.data() : nullptr, w_, h_, &p, &p),
           ctx_);
     color_lum2.clear(), background_lum2.clear();
+  }
+  // Any of the filters above on a panorama's film, periodic in x (rayn_b200_film_denoise_wrap): sigma_luminance = +inf is the
+  // filter without the variance term, with_albedo adds the albedo guide of render_albedo.
+  void denoise_wrap(int iterations, float sigma_color, float sigma_normal, float sigma_alpha, float sigma_luminance, bool with_albedo,
+                    float sigma_albedo) {
+    const bool var = !std::isinf(sigma_luminance);
+    if (var && color_lum2.empty()) throw std::runtime_error("denoise_wrap with the variance term needs a render_frame_into(..., moments = true) first");
+    if (with_albedo && albedo.empty()) throw std::runtime_error("denoise_wrap with the albedo guide needs render_albedo first");
+    const RaynDenoiseDesc d{iterations, sigma_color, sigma_normal, sigma_alpha};
+    RaynFilmPlanes p{color.data(), alpha.data(), background.data(), normal.data(), RAYN_MEM_HOST};
+    const RaynMomentPlanes m{color_lum2.data(), background_lum2.data(), RAYN_MEM_HOST};
+    check(rayn_b200_film_denoise_wrap(ctx_, &d, sigma_luminance, spp_, var ? &m : nullptr, nullptr, sigma_albedo,
+                                      with_albedo ? albedo.data() : nullptr, w_, h_, &p, &p),
+          ctx_);
+    if (var) color_lum2.clear(), background_lum2.clear();
   }
   int width() const { return w_; }
   int height() const { return h_; }

@@ -396,6 +396,25 @@ class OrthographicCamera(_Camera):  # camera.rs:227-241
         return c
 
 
+class EquirectangularCamera(_Camera):
+    """A 360-degree equirectangular panorama (include/rayn_b200.h, RAYN_CAMERA_EQUIRECTANGULAR): an EXTENSION with no
+    reference counterpart.  u spans the full turn about `up` (the screen centre looks at `at`), v runs from the -up pole to the
+    +up pole; origin, at and up may each be a constant, Linear or a closure, as for PinholeCamera.  Its film is periodic in x:
+    Film denoises and accumulates it across the seam."""
+
+    def __init__(self, resolution, origin, at, up):
+        self.res = (f32(resolution[0]), f32(resolution[1]))
+        self.half_pixel_size = f32(f32(math.pi) / self.res[1]) / f32(2.0)  # the angular half pixel
+        self.origin, self.at, self.up = _seq(origin), _seq(at), _seq(up)
+
+    def flatten(self, time_range=None):
+        c = L.RaynCamera()
+        c.kind = L.CAMERA_EQUIRECTANGULAR
+        c.half_pixel_size = float(self.half_pixel_size)
+        _store_seq(c, time_range, self.origin, self.at, self.up)
+        return c
+
+
 class CameraStore:  # camera.rs:24-40
     def __init__(self):
         self.items = []
