@@ -90,13 +90,35 @@ typedef enum RaynMaterialKind {
   RAYN_MATERIAL_LAMBERTIAN = 0, /* src/material.rs:86-142                                   */
   RAYN_MATERIAL_DIELECTRIC = 1, /* src/material.rs:144-257; roughness = REMAPPED exponent   */
   RAYN_MATERIAL_SKY = 2,        /* src/material.rs:394-449                                  */
-  RAYN_MATERIAL_EMISSIVE = 3    /* src/material.rs:451-520                                  */
+  RAYN_MATERIAL_EMISSIVE = 3,   /* src/material.rs:451-520                                  */
+  RAYN_MATERIAL_METALLIC = 4    /* EXTENSION, no reference counterpart: a glossy conductor, below */
 } RaynMaterialKind;
+
+/* ---- Metallic: a glossy conductor with coloured Fresnel, an EXTENSION with no reference counterpart ----------------------
+ * The Dielectric's specular lobe with F0 per channel and no diffuse term.  albedo[3] holds F0 (finite), roughness the Phong
+ * exponent after new_remap exactly as for the Dielectric (finite, > 0); upload_scene refuses anything else with
+ * RAYN_ERR_INVALID_ARG.  In float with the build's mul_add (dot / normalized / reflected / onb / cosine_power / dm::pow as
+ * the Dielectric uses them in rt_device.cuh), rough = roughness, f_schlick(c, f0) = f0 + (1 - f0) * powi5(1 - c),
+ * pi_f = 3.14159265f, 2pi_f = 6.28318531f:
+ *   f(first, second, n), called as bsdf.f(wo, wi, n) like the other kinds (integrator.rs:230):
+ *     dotv = max(0, dot(first, n)),  half = normalized(second + first),  cos_alpha = dm::pow(max(0, dot(half, n)), rough)
+ *     spec_factor = cos_alpha * (rough + 2) / (2 * pi_f),  f[c] = spec_factor * f_schlick(dotv, F0[c])
+ *   scatter(wo, sp, s1d, u0, u1, u2, u3): the Dielectric's specular branch (material.rs:207-256), always taken:
+ *     cosv = |dot(n, wo)|,  spec_sample = cosine_power(u2, u3, rough),  spec_bounce = normalized(onb(reflected(wo, n)) * spec_sample)
+ *     cos_alpha_pow = max(dm::pow(spec_sample.z, rough), FLT_EPSILON)
+ *     spec_pdf = (rough + 1) / 2pi_f * cos_alpha_pow,  spec_coeff = (rough + 2) / 2pi_f * cos_alpha_pow, 0 if dot(n, spec_bounce) < 0
+ *     wi = spec_bounce,  f[c] = spec_coeff * f_schlick(cosv, F0[c]),  pdf = spec_pdf
+ *   s1d, u0 and u1 are not read: the metal draws from the same sample dimensions as the other kinds.
+ * A metal receives light like Lambertian and Dielectric: next-event estimation, the alpha and normal channels, roulette and
+ * the shadow rays.  An orbit-trap palette (RaynAlbedoTrap) replaces F0 wherever the BSDF reads it, and the first-hit albedo
+ * plane gives F0 (or the palette).  For finite inputs (tested):
+ *   (a) F0 = (0.04, 0.04, 0.04): f equals a Dielectric's f with albedo (0, 0, 0) and the same exponent, bit for bit;
+ *   (b) F0 = (1, 1, 1): scatter's wi and f equal a Dielectric's with s1d = 0 (its specular lobe), bit for bit; the pdf differs. */
 
 typedef struct RaynMaterial {
   int32_t kind;
-  float albedo[3];     /* Lambertian / Dielectric                                          */
-  float roughness;     /* Dielectric: the Phong exponent AFTER new_remap (material.rs:167-174) */
+  float albedo[3];     /* Lambertian / Dielectric; Metallic: F0 per channel                 */
+  float roughness;     /* Dielectric, Metallic: the Phong exponent AFTER new_remap (material.rs:167-174) */
   float sky_top[3];    /* Sky::new(top, bottom)                                            */
   float sky_bottom[3];
   float emission[3];   /* Emissive::new_splat                                              */
@@ -118,11 +140,12 @@ typedef struct RaynMaterial {
  *           a hit on an analytic sphere whose material has a trap has s = 1 (no orbit)
  *   albedo  albedo[c] = albedo_lo[c] * (1 - s) + albedo_hi[c] * s, with (1 - s) computed once
  * The albedo replaces RaynMaterial.albedo wherever that hit's BSDF reads it: the Lambertian f and scatter f, and the
- * Dielectric diffuse term of f (next-event estimation) and of scatter.  Normals, offsets, sample dimensions, packet
+ * Dielectric diffuse term of f (next-event estimation) and of scatter; for a Metallic it replaces F0 in f and scatter.
+ * Normals, offsets, sample dimensions, packet
  * composition, light choice and the alpha / normal channels do not change; trap evaluations are not counted in
  * RaynStats.sdf_evals_normals.                                                                                      */
 typedef struct RaynAlbedoTrap {
-  int32_t material;                 /* index into the uploaded scene's materials: LAMBERTIAN or DIELECTRIC, one entry per material */
+  int32_t material;                 /* index into the uploaded scene's materials: LAMBERTIAN, DIELECTRIC or METALLIC, one per material */
   float trap_lo, trap_hi;           /* finite, trap_lo < trap_hi                                                                   */
   float albedo_lo[3], albedo_hi[3]; /* finite                                                                                      */
 } RaynAlbedoTrap;
@@ -363,7 +386,7 @@ int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* fr
  * lane 0 of its 4-sample packet) is traced to its closest hit with the DEPTH-0 fold of render_frame (hitable.rs:170-198,
  * threshold film.rs:540-551), which is render_frame's depth-0 hit exactly (moving spheres at lane 0's time of the extend
  * packet, which at depth 0 is samples 4k..4k+3 of the pixel).  Its albedo a_s is
- *   Lambertian or Dielectric hit: the albedo the BSDF reads at depth 0, i.e. RaynMaterial.albedo, or for a material with
+ *   Lambertian, Dielectric or Metallic hit: the albedo the BSDF reads at depth 0 (F0 for a metal), i.e. RaynMaterial.albedo, or for a material with
  *     an orbit trap lo*(1 - s') + hi*s' (RaynAlbedoTrap) with s' = trap_coord(trap(p)), p = dir.mul_add(t, origin) the hit
  *     point (ray.rs:22-24), s' = 1 on an analytic sphere;
  *   Sky or Emissive hit, or nothing hit: (0, 0, 0).
@@ -372,9 +395,9 @@ int32_t rayn_b200_render_frame_moments(RaynContext* ctx, const RaynFrameDesc* fr
  * other frame checks are render_frame's.  RAYN_FLAG_SIMPLE_MARCH: RAYN_ERR_UNSUPPORTED.  Synchronous; replaces RaynStats
  * like a render (k_first_hit_paths counts under RAYN_K_NORMALS, k_albedo_resolve under RAYN_K_RESOLVE); never captured
  * into a CUDA graph, and later renders are unaffected.
- * Property (tested): if every Lambertian / Dielectric material has albedo (1, 1, 1) and there are no traps, every channel
- * equals render_frame's alpha plane bit for bit, for the same frame: alpha is nA / spp with nA the count of depth-0
- * Lambertian / Dielectric hits, and a sum of nA ones is nA exactly.                                                 */
+ * Property (tested): if every Lambertian / Dielectric / Metallic material has albedo (F0) (1, 1, 1) and there are no traps,
+ * every channel equals render_frame's alpha plane bit for bit, for the same frame: alpha is nA / spp with nA the count of
+ * depth-0 Lambertian / Dielectric / Metallic hits, and a sum of nA ones is nA exactly.                                                 */
 int32_t rayn_b200_render_albedo(RaynContext* ctx, const RaynFrameDesc* frame, float* albedo /* [3*W*H] */, int32_t space);
 
 /* ---- screen-space motion of the first hit: the reprojection input of rayn_b200_temporal_push ----------------------------

@@ -34,6 +34,7 @@ COMM_ID_BYTES = 128
 
 HITABLE_SPHERE, HITABLE_MANDELBOX, HITABLE_MANDELBULB = 0, 1, 2
 MATERIAL_LAMBERTIAN, MATERIAL_DIELECTRIC, MATERIAL_SKY, MATERIAL_EMISSIVE = 0, 1, 2, 3
+MATERIAL_METALLIC = 4  # EXTENSION, no reference counterpart (include/rayn_b200.h)
 CAMERA_PINHOLE, CAMERA_THINLENS, CAMERA_ORTHOGRAPHIC, CAMERA_EQUIRECTANGULAR = 0, 1, 2, 3
 MEM_HOST, MEM_DEVICE = 0, 1
 POST_COLOR_PLUS_BACKGROUND, POST_COLOR_ALPHA, POST_COLOR_ONLY, POST_BACKGROUND, POST_WORLD_NORMAL, POST_ALPHA = range(6)

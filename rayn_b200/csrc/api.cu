@@ -100,6 +100,7 @@ struct RaynContext {
   int occ_ext[2][SDFV_COUNT], occ_shd[SDFV_COUNT], occ_nrm[SDFV_COUNT], occ_nrm_trap[SDFV_COUNT];  // occ_ext[constant threshold][variant]
   int occ_pre = 8, occ_post = 8, occ_sph = 8;  // resident CTAs per SM of the work-list kernels
   int occ_pre_trap = 8, occ_post_trap = 8;     // ... of the shading kernels of scenes with orbit-trap albedos
+  int occ_pre_metal[2] = {8, 8}, occ_post_metal[2] = {8, 8};  // ... of scenes with a Metallic material, [without / with traps]
   int sdf_var[RAYN_MAX_HITABLES];  // march-kernel variant of every SDF hitable of the uploaded scene (rt_sdf2.cuh::sdf_variant)
   struct Div3Check { float min_r2, fixed_r2; bool ok; };
   std::vector<Div3Check> div3_cache;  // exhaustive fastdiv2_3 checks already run on this device
@@ -391,6 +392,10 @@ int32_t rayn_b200_create(const RaynConfig* cfg, RaynContext** out_ctx) {
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post, k_shade_post<false>, SLOT_BLOCK, 0);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre_trap, k_shade_pre<true>, SLOT_BLOCK, 0);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post_trap, k_shade_post<true>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre_metal[0], k_shade_pre<false, true>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post_metal[0], k_shade_post<false, true>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_pre_metal[1], k_shade_pre<true, true>, SLOT_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_post_metal[1], k_shade_post<true, true>, SLOT_BLOCK, 0);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_sph, k_extend_spheres, EXT_BATCH, 0);
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -460,9 +465,15 @@ static int32_t validate_scene(RaynContext* ctx, const RaynSceneDesc* s) {
     if (h.kind == RAYN_HITABLE_MANDELBULB && h.bulb_power != 8)
       return fail(ctx, RAYN_ERR_UNSUPPORTED, "hitable %d: Mandelbulb power %d (only 8 is built)", i, h.bulb_power);
   }
-  for (int i = 0; i < s->n_materials; ++i)
-    if (s->materials[i].kind < 0 || s->materials[i].kind > RAYN_MATERIAL_EMISSIVE)
-      return fail(ctx, RAYN_ERR_INVALID_ARG, "material %d: bad kind %d", i, s->materials[i].kind);
+  for (int i = 0; i < s->n_materials; ++i) {
+    const RaynMaterial& m = s->materials[i];
+    if (m.kind < 0 || m.kind > RAYN_MATERIAL_METALLIC) return fail(ctx, RAYN_ERR_INVALID_ARG, "material %d: bad kind %d", i, m.kind);
+    if (m.kind == RAYN_MATERIAL_METALLIC) {
+      const bool finite = std::isfinite(m.albedo[0]) && std::isfinite(m.albedo[1]) && std::isfinite(m.albedo[2]) && std::isfinite(m.roughness);
+      if (!finite) return fail(ctx, RAYN_ERR_INVALID_ARG, "material %d: Metallic with a non-finite F0 or exponent", i);
+      if (!(m.roughness > 0.0f)) return fail(ctx, RAYN_ERR_INVALID_ARG, "material %d: Metallic exponent %g is not > 0", i, m.roughness);
+    }
+  }
   if (s->camera.kind < 0 || s->camera.kind > RAYN_CAMERA_EQUIRECTANGULAR) return fail(ctx, RAYN_ERR_INVALID_ARG, "bad camera kind");
   if (s->consts.max_marches < 1 || s->consts.max_vis_marches < 1) return fail(ctx, RAYN_ERR_INVALID_ARG, "march limits must be >= 1");
   return RAYN_OK;
@@ -541,8 +552,8 @@ int32_t rayn_b200_set_albedo_traps(RaynContext* ctx, int32_t n, const RaynAlbedo
     const int m = t.material;
     if (m < 0 || m >= ctx->scene.n_mat) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d out of range", i, m);
     const int mk = ctx->scene.mat[m].kind;
-    if (mk != RAYN_MATERIAL_LAMBERTIAN && mk != RAYN_MATERIAL_DIELECTRIC)
-      return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d is neither Lambertian nor Dielectric", i, m);
+    if (mk != RAYN_MATERIAL_LAMBERTIAN && mk != RAYN_MATERIAL_DIELECTRIC && mk != RAYN_MATERIAL_METALLIC)
+      return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d is not Lambertian, Dielectric or Metallic", i, m);
     if (mask & (1u << m)) return fail(ctx, RAYN_ERR_INVALID_ARG, "trap %d: material %d has a trap already", i, m);
     bool finite = std::isfinite(t.trap_lo) && std::isfinite(t.trap_hi);
     for (int c = 0; c < 3; ++c) finite = finite && std::isfinite(t.albedo_lo[c]) && std::isfinite(t.albedo_hi[c]);
@@ -588,7 +599,7 @@ int64_t rayn_b200_debug_read_queue_log(RaynContext* ctx, int32_t* out, int64_t c
 struct FramePlan {
   DevFrame fr;
   int R, QS, np, wpc;  // paths and shading slots per tile; k_resolve's padded spp and warps per CTA
-  bool simple, traps, fold_all, volume_on;
+  bool simple, traps, metal, fold_all, volume_on;
   int fold_pre, n_fold, ns, seg_per_path, lc_ns;
 };
 
@@ -688,6 +699,8 @@ static int32_t scene_plan(RaynContext* ctx, FramePlan* P) {
   if (motion && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "time-varying sphere centres are not supported by the legacy test kernels");
   const bool traps = P->traps = ctx->scene.trap_mask != 0u;
   if (traps && simple) return fail(ctx, RAYN_ERR_UNSUPPORTED, "orbit-trap albedos are not supported by the legacy test kernels");
+  P->metal = false;  // a Metallic material: the shading kernels with the metal branches (rt_device.cuh::receives_light)
+  for (int m = 0; m < ctx->scene.n_mat; ++m) P->metal = P->metal || ctx->scene.mat[m].kind == RAYN_MATERIAL_METALLIC;
   // leading analytic spheres run inside raygen / shade_post (rt_kernels.cuh::fold_head); -1 = not folded (moving spheres need
   // the extend packet's lane-0 time; the legacy test kernels do the whole fold themselves)
   int& fold_pre = P->fold_pre;
@@ -921,7 +934,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   const bool mom = moments != nullptr;
   const int mb = fr.max_bounces, np = P.np, wpc = mom ? resolve_warps_per_cta(np, true) : P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
   const int* sdf_idx = ctx->scene.sdf_idx;
-  const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, volume_on = P.volume_on;
+  const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, metal = P.metal, volume_on = P.volume_on;
 
   if (mom && wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
   const size_t npx = (size_t)f->width * f->height;
@@ -1045,7 +1058,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
         for (int j = 0; j < n_sdf; ++j) {
           const RaynHitable& h = ctx->scene.hit[sdf_idx[j]];
           const int mk = ctx->scene.mat[h.material].kind;
-          if (!(mk == RAYN_MATERIAL_LAMBERTIAN || mk == RAYN_MATERIAL_DIELECTRIC || volume_on)) continue;
+          if (!(mk == RAYN_MATERIAL_LAMBERTIAN || mk == RAYN_MATERIAL_DIELECTRIC || mk == RAYN_MATERIAL_METALLIC || volume_on)) continue;
           const int v = ctx->sdf_var[sdf_idx[j]];
           timed_begin(ctx, RAYN_K_NORMALS);
           if ((ctx->scene.trap_mask >> h.material) & 1u)  // the bin's material has an orbit-trap albedo: normals + trap
@@ -1055,7 +1068,11 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           timed_end(ctx, RAYN_K_NORMALS);
         }
         timed_begin(ctx, RAYN_K_SHADE_PRE);
-        if (traps)
+        if (metal && traps)
+          k_shade_pre<true, true><<<resident(ctx, J, ctx->occ_pre_metal[1]), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
+        else if (metal)
+          k_shade_pre<false, true><<<resident(ctx, J, ctx->occ_pre_metal[0]), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
+        else if (traps)
           k_shade_pre<true><<<resident(ctx, J, ctx->occ_pre_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
         else
           k_shade_pre<false><<<resident(ctx, J, ctx->occ_pre), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, thr, J.work_ctr + WC_PRE);
@@ -1069,7 +1086,11 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           }
         }
         timed_begin(ctx, RAYN_K_SHADE_POST);
-        if (traps)
+        if (metal && traps)
+          k_shade_post<true, true><<<resident(ctx, J, ctx->occ_post_metal[1]), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);
+        else if (metal)
+          k_shade_post<false, true><<<resident(ctx, J, ctx->occ_post_metal[0]), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);
+        else if (traps)
           k_shade_post<true><<<resident(ctx, J, ctx->occ_post_trap), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);
         else
           k_shade_post<false><<<resident(ctx, J, ctx->occ_post), SLOT_BLOCK, 0, st>>>(ctx->scene, fr, pb, depth, n_fold, J.work_ctr + WC_POST);

@@ -503,7 +503,11 @@ RT_D void light_sample_volume(const RaynLight& L, float sample, f3 ray_o, f3 ray
 }
 
 // ---- BSDFs, material.rs ---------------------------------------------------------------------------
+// METAL = false: the caller's scene has no Metallic material (api.cu picks the shading kernels by it), so the kind test and
+// the metal branches below are not compiled in and those kernels are the code scenes without metals always ran.
+template <bool METAL = true>
 RT_D bool receives_light(const RaynMaterial& m) {
+  if constexpr (METAL) return m.kind == RAYN_MATERIAL_LAMBERTIAN || m.kind == RAYN_MATERIAL_DIELECTRIC || m.kind == RAYN_MATERIAL_METALLIC;
   return m.kind == RAYN_MATERIAL_LAMBERTIAN || m.kind == RAYN_MATERIAL_DIELECTRIC;
 }
 RT_D f3 bsdf_le(const RaynMaterial& m, f3 wo) {
@@ -514,11 +518,48 @@ RT_D f3 bsdf_le(const RaynMaterial& m, f3 wo) {
   if (m.kind == RAYN_MATERIAL_EMISSIVE) return ld3(m.emission);  // :517-519
   return {0.0f, 0.0f, 0.0f};
 }
+struct Scatter {
+  f3 wi, f;
+  float pdf;
+};
+// Metallic (EXTENSION, no reference counterpart; statement in include/rayn_b200.h): the Dielectric's specular lobe below with
+// F0 per channel and no diffuse term.  f is the Dielectric's f without the diffuse term, with f_schlick(dotv, F0[c]).
+RT_D f3 metal_f(float rough, f3 f0, f3 first, f3 second, f3 n) {
+  const float dotv = dm::max(0.0f, dot(first, n));
+  const f3 half = normalized(second + first);
+  const float cos_alpha = dm::pow(dm::max(0.0f, dot(half, n)), rough);
+  const float spec_factor = cos_alpha * (rough + 2.0f) / (2.0f * RT_PI);
+  return {spec_factor * f_schlick(dotv, f0.x), spec_factor * f_schlick(dotv, f0.y), spec_factor * f_schlick(dotv, f0.z)};
+}
+// scatter is the Dielectric's specular branch, operation for operation, always taken; s1d, u0 and u1 are not read
+RT_D Scatter metal_scatter(float rough, f3 f0, f3 wo, const ShadingPoint& sp, float u2, float u3) {
+  const f3 norm = sp.normal;
+  const float cosv = dm::abs(dot(norm, wo));
+  const f3 spec_sample = cosine_power(u2, u3, rough);
+  const f3 reflection = reflected(wo, norm);
+  const m3 basis = onb(reflection);
+  const f3 spec_bounce = normalized(mul(basis, spec_sample));
+  const float cos_alpha_pow = dm::max(dm::pow(spec_sample.z, rough), RT_EPSILON);
+  const float spec_pdf = (rough + 1.0f) / RT_TWO_PI * cos_alpha_pow;
+  float spec_coeff = (rough + 2.0f) / RT_TWO_PI * cos_alpha_pow;
+  const bool below_horizon = dot(norm, spec_bounce) < 0.0f;
+  spec_coeff = below_horizon ? 0.0f : spec_coeff;
+  Scatter se;
+  se.wi = spec_bounce;
+  se.f = mk3(spec_coeff * f_schlick(cosv, f0.x), spec_coeff * f_schlick(cosv, f0.y), spec_coeff * f_schlick(cosv, f0.z));
+  se.pdf = spec_pdf;
+  return se;
+}
+
 // called as bsdf.f(wo, wi, n) (integrator.rs:230); see oracle note on argument naming.  `albedo` is what the material's
-// albedo generator gives at this hit: m.albedo, or an orbit-trap palette (trap_albedo).
+// albedo generator gives at this hit: m.albedo, or an orbit-trap palette (trap_albedo); a Metallic reads it as F0.
+template <bool METAL = true>
 RT_D f3 bsdf_f(const RaynMaterial& m, f3 albedo, f3 first, f3 second, f3 n) {
   if (m.kind == RAYN_MATERIAL_LAMBERTIAN) return albedo / RT_PI;  // :139-141
-  float rough = m.roughness;                                      // Dielectric :195-205
+  if constexpr (METAL) {
+    if (m.kind == RAYN_MATERIAL_METALLIC) return metal_f(m.roughness, albedo, first, second, n);
+  }
+  float rough = m.roughness;  // Dielectric :195-205
   float dotv = dm::max(0.0f, dot(first, n));
   float fresnel = f_schlick(dotv, 0.04f);
   f3 half = normalized(second + first);
@@ -528,13 +569,13 @@ RT_D f3 bsdf_f(const RaynMaterial& m, f3 albedo, f3 first, f3 second, f3 n) {
   f3 diffuse_f = albedo / RT_PI * (1.0f - fresnel);
   return spec_f + diffuse_f;
 }
-RT_D f3 bsdf_f(const RaynMaterial& m, f3 first, f3 second, f3 n) { return bsdf_f(m, ld3(m.albedo), first, second, n); }
-struct Scatter {
-  f3 wi, f;
-  float pdf;
-};
+RT_D f3 bsdf_f(const RaynMaterial& m, f3 first, f3 second, f3 n) { return bsdf_f<true>(m, ld3(m.albedo), first, second, n); }
+template <bool METAL = true>
 RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 albedo, f3 wo, const ShadingPoint& sp, float s1d, float u0, float u1, float u2,
                           float u3) {
+  if constexpr (METAL) {
+    if (m.kind == RAYN_MATERIAL_METALLIC) return metal_scatter(m.roughness, albedo, wo, sp, u2, u3);
+  }
   Scatter se;
   if (m.kind != RAYN_MATERIAL_DIELECTRIC) {  // Lambertian :118-137 (Emissive/Sky never scatter on the path)
     f3 ds = cosine_weighted(u0, u1);
@@ -569,7 +610,7 @@ RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 albedo, f3 wo, const Shading
   return se;
 }
 RT_D Scatter bsdf_scatter(const RaynMaterial& m, f3 wo, const ShadingPoint& sp, float s1d, float u0, float u1, float u2, float u3) {
-  return bsdf_scatter(m, ld3(m.albedo), wo, sp, s1d, u0, u1, u2, u3);
+  return bsdf_scatter<true>(m, ld3(m.albedo), wo, sp, s1d, u0, u1, u2, u3);
 }
 
 RT_D int light_index(float s, int n_lights) {  // integrator.rs:76-77 (+ clamp, A10)

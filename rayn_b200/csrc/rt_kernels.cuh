@@ -691,6 +691,7 @@ struct LightContrib {
 };
 // round 0: surface_sample_one_light (integrator.rs:207-240) without the visibility factor;
 // round r>0: volume_sample_one_light (:242-281) for volume march r-1.
+template <bool METAL>
 RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, f3 albedo, const ShadingPoint& sp, f3 wo, int round, float u0,
                                 float u1, float vol_sample, bool has_ext, float neg_rho_t) {
   LightContrib r;
@@ -703,7 +704,7 @@ RT_D LightContrib light_contrib(const RaynLight& L, const RaynMaterial& mat, f3 
     const float dist = mag(wi);
     wi = wi / dist;
     r.start = sp.point + sp.normal * dm::signum(dot(sp.normal, wi)) * sp.offset_by;
-    const f3 f = bsdf_f(mat, albedo, wo, wi, sp.normal) * dm::max(dot(sp.normal, wi), 0.0f);
+    const f3 f = bsdf_f<METAL>(mat, albedo, wo, wi, sp.normal) * dm::max(dot(sp.normal, wi), 0.0f);
     const float tr = has_ext ? dm::exp(neg_rho_t * dist) : 1.0f;
     r.c = li * f * tr;
     r.den = pdf;
@@ -777,7 +778,7 @@ RT_D SlotCtx slot_ctx(const DevScene& sc, const DevFrame& fr, const PassBufs& pb
   return c;
 }
 
-template <bool TRAP>
+template <bool TRAP, bool METAL>
 RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs& pb, const int depth, const Thr thr, const int ts, const int s) {
   const int nslots = pb.n_slots[ts];
   if ((s & ~31) >= nslots) return;  // warp-uniform
@@ -799,7 +800,7 @@ RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs&
     sp.d = mk3(d4.x, d4.y, d4.z);
     sp.time = o4.w;
     sp.t = d4.w;
-    const bool recv = receives_light(mat);
+    const bool recv = receives_light<METAL>(mat);
     const int nl = sc.n_lights;
     const bool scat = sc.vol.has_scattering != 0 && nl > 0;
     const int n_rounds = nl > 0 ? 1 + (scat ? fr.vm : 0) : 0;
@@ -834,7 +835,7 @@ RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs&
 #pragma unroll 1
         for (int i = 0; i < 4; ++i) {
           const int set = round == 0 ? cx.set2 + i : cx.set2 + 4 + 4 * (round - 1) + i;
-          const LightContrib lc = light_contrib(sc.light[(wr >> (8 * i)) & 0xffu], mat, TRAP ? tr_albedo : ld3(mat.albedo), sp, wo, round, samp2(fr, 0, cx.sample, cx.scramble, set),
+          const LightContrib lc = light_contrib<METAL>(sc.light[(wr >> (8 * i)) & 0xffu], mat, TRAP ? tr_albedo : ld3(mat.albedo), sp, wo, round, samp2(fr, 0, cx.sample, cx.scramble, set),
                                                 samp2(fr, 1, cx.sample, cx.scramble, set), vol_sample, has_ext, neg_rho_t);
           ++shadows;
           const int bit = round * 4 + i;
@@ -878,12 +879,14 @@ RT_D void shade_pre_slot(const DevScene& sc, const DevFrame& fr, const PassBufs&
 #ifndef RAYN_SHADE_PRE_OCC
 #define RAYN_SHADE_PRE_OCC 8  // resident CTAs per SM k_shade_pre is compiled for (tuning hook)
 #endif
-// TRAP: the scene has orbit-trap albedos (DevScene::trap_mask != 0); the TRAP = false kernel is the one scenes without traps run
-template <bool TRAP>
+// TRAP: the scene has orbit-trap albedos (DevScene::trap_mask != 0); the TRAP = false kernel is the one scenes without traps run.
+// METAL: the scene has a Metallic material (rt_device.cuh::receives_light); the METAL = false kernels are the ones scenes without
+// metals run, the same code as before the material existed.
+template <bool TRAP, bool METAL = false>
 __global__ void __launch_bounds__(128, RAYN_SHADE_PRE_OCC) k_shade_pre(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb,
                                                       const int depth, const Thr thr, int* __restrict__ work_ctr) {
   // row 0 of the work lists: the non-empty 128-slot blocks of every tile's shading queue
-  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_pre_slot<TRAP>(sc, fr, pb, depth, thr, ts, local * SLOT_BLOCK + threadIdx.x); })
+  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_pre_slot<TRAP, METAL>(sc, fr, pb, depth, thr, ts, local * SLOT_BLOCK + threadIdx.x); })
 }
 // k_shade_pre has the largest parameter list of the render kernels.  The scene limits of include/rayn_b200.h are sized for the
 // 4 KB kernel-parameter block; the orbit-trap palettes (DevScene::trap) leave little of it, so a later addition fails here.
@@ -1001,7 +1004,7 @@ __global__ void __launch_bounds__(SHD_T, MARCH_OCC(V)) k_shadow(const __grid_con
   if (V == SDFV_BULB) warp_add(pb.counters + CNT_BULB_ITERS_SHADOW, bulb_iters);
 }
 
-template <bool TRAP>
+template <bool TRAP, bool METAL>
 RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs& pb, const int depth, const int pre_n, const int ts, const int s) {
   const int nslots = pb.n_slots[ts];
   if ((s & ~31) >= nslots) return;
@@ -1026,7 +1029,7 @@ RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs
   const bool has_ext = sc.vol.has_extinction != 0;
   const float neg_rho_t = -sc.vol.coeff_extinction;
   const float vt = has_ext ? dm::exp(neg_rho_t * sp.t) : 1.0f;
-  const bool recv = receives_light(mat);
+  const bool recv = receives_light<METAL>(mat);
   const int nl = sc.n_lights;
   const bool scat = sc.vol.has_scattering != 0 && nl > 0;
   const int n_rounds = nl > 0 ? 1 + (scat ? fr.vm : 0) : 0;
@@ -1052,7 +1055,7 @@ RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs
   }
   if (recv) {  // :134-188
     const int setb = cx.set2 + 4 + 4 * fr.vm;
-    const Scatter se = bsdf_scatter(mat, TRAP ? hit_albedo(sc, pb, h, mat, g) : ld3(mat.albedo), wo, sp, samp1(fr, cx.sample, cx.scramble, cx.set1 + 3),
+    const Scatter se = bsdf_scatter<METAL>(mat, TRAP ? hit_albedo(sc, pb, h, mat, g) : ld3(mat.albedo), wo, sp, samp1(fr, cx.sample, cx.scramble, cx.set1 + 3),
                                     samp2(fr, 0, cx.sample, cx.scramble, setb),
                                     samp2(fr, 1, cx.sample, cx.scramble, setb), samp2(fr, 0, cx.sample, cx.scramble, setb + 1),
                                     samp2(fr, 1, cx.sample, cx.scramble, setb + 1));
@@ -1088,10 +1091,10 @@ RT_D void shade_post_slot(const DevScene& sc, const DevFrame& fr, const PassBufs
   }
 }
 
-template <bool TRAP>
+template <bool TRAP, bool METAL = false>
 __global__ void __launch_bounds__(128, 8) k_shade_post(const __grid_constant__ DevScene sc, const DevFrame fr, const PassBufs pb,
                                                        const int depth, const int pre_n, int* __restrict__ work_ctr) {
-  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_post_slot<TRAP>(sc, fr, pb, depth, pre_n, ts, local * SLOT_BLOCK + threadIdx.x); })
+  FOR_EACH_WORK_BLOCK(pb.slot_prefix, pb.n_tiles, work_ctr, { shade_post_slot<TRAP, METAL>(sc, fr, pb, depth, pre_n, ts, local * SLOT_BLOCK + threadIdx.x); })
 }
 
 // ------------------------------------------------------------------------------------------

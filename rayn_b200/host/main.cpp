@@ -1,11 +1,14 @@
 // main.cpp — stand-in for rayn's src/main.rs + src/setup.rs on top of the C ABI.
 //   rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] [--denoise L]
-//             [--denoise-albedo] [--denoise-variance] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--panorama] [--out file.ppm] [--dump planes.bin]
+//             [--denoise-albedo] [--denoise-variance] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--metallic R G B ROUGHNESS] [--panorama]
+//             [--out file.ppm] [--dump planes.bin]
 // --denoise-albedo (with --denoise) renders the first-hit albedo plane as rayn_b200.film.Film does and guides the filter with it.
 // --denoise-variance (with --denoise, not with --adaptive) renders the frame with its luminance moments and weights each
 // pixel's colour by its own variance, as rayn_b200.film.Film does with a "moments" channel; combinable with --denoise-albedo.
 // --orbit-trap colours the fractal of configs 2-5 by orbit trap: albedo (R0 G0 B0) at trap LO, (R1 G1 B1) at HI
 // (include/rayn_b200.h, RaynAlbedoTrap; tools/trap_range.py prints a range for config 3).
+// --metallic replaces the fractal's material (the sphere's in config 1) with Metallic::new_remap(Srgb(R, G, B), ROUGHNESS), a
+// glossy conductor with F0 = (R G B) (include/rayn_b200.h, RAYN_MATERIAL_METALLIC); with --orbit-trap the palette replaces F0.
 // --panorama replaces the config's camera with a 360-degree equirectangular one at the same origin, at and up (include/rayn_b200.h,
 // RAYN_CAMERA_EQUIRECTANGULAR), as rayn_b200.EquirectangularCamera; --denoise then filters across the seam
 // (rayn_b200_film_denoise_wrap).  W must leave no partial tile narrower than half a tile (the reference tile grid drops it).
@@ -37,12 +40,21 @@ static constexpr int kAdaptiveMaxRounds = 32;
 
 // setup.rs:46-169; `fractal` 0 = Mandelbox (the reference scene), 1 = authored Mandelbulb
 // trap: the fractal's albedo generator (--orbit-trap), NULL = the reference's constant grey
-static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens, const OrbitTrapAlbedo* trap = nullptr) {
+// metal: the fractal's (F0, roughness) as a Metallic (--metallic), NULL = the reference's Dielectric
+struct MetalArgs {
+  Srgb f0;
+  float roughness;
+};
+static Material fractal_material(const OrbitTrapAlbedo* trap, const MetalArgs* metal) {
+  if (metal) return trap ? Material(Metallic::new_remap(*trap, metal->roughness)) : Material(Metallic::new_remap(metal->f0, metal->roughness));
+  return trap ? Material(Dielectric::new_remap(*trap, 0.6f)) : Material(Dielectric::new_remap(Srgb(0.2f, 0.2f, 0.2f), 0.6f));  // :76
+}
+static CameraHandle setup(World& world, float rx, float ry, bool volume, int fractal, bool thinlens, const OrbitTrapAlbedo* trap = nullptr,
+                          const MetalArgs* metal = nullptr) {
   if (volume) world.volume_params = VolumeParams{true, true, 0.25f, 0.035f};                      // :55-60
   const MaterialHandle sky = world.materials.add_material(Sky(Srgb(0.3f, 0.4f, 0.6f), Srgb(0.2f, 0.3f, 0.6f) * 0.05f));  // :63-69
   world.hitables.push(Sphere(Vec3(0, 0, 0), WORLD_RADIUS, sky));                                  // :71
-  const MaterialHandle grey = trap ? world.materials.add_material(Dielectric::new_remap(*trap, 0.6f))
-                                   : world.materials.add_material(Dielectric::new_remap(Srgb(0.2f, 0.2f, 0.2f), 0.6f));  // :76
+  const MaterialHandle grey = world.materials.add_material(fractal_material(trap, metal));  // :76
   if (fractal == 0)
     world.hitables.push(TracedSDF(MandelBox(FRACTAL_ITERATIONS, BoxFold(1.0f), SphereFold(0.01f, 1.9f), -2.1f), grey));  // :78-86
   else
@@ -66,10 +78,10 @@ static CameraHandle setup(World& world, float rx, float ry, bool volume, int fra
   return world.cameras.add_camera(PinholeCamera(rx, ry, 60.0f, origin, Vec3(0, 0, 0), Vec3(0, 1, 0)));  // :129-141
 }
 
-static CameraHandle setup_single_sphere(World& world, float rx, float ry) {  // BASELINE config 1
+static CameraHandle setup_single_sphere(World& world, float rx, float ry, const MetalArgs* metal = nullptr) {  // BASELINE config 1
   const MaterialHandle sky = world.materials.add_material(Sky(Srgb(0.3f, 0.4f, 0.6f), Srgb(0.2f, 0.3f, 0.6f) * 0.05f));
   world.hitables.push(Sphere(Vec3(0, 0, 0), WORLD_RADIUS, sky));
-  const MaterialHandle grey = world.materials.add_material(Dielectric::new_remap(Srgb(0.2f, 0.2f, 0.2f), 0.6f));
+  const MaterialHandle grey = world.materials.add_material(fractal_material(nullptr, metal));
   world.hitables.push(Sphere(Vec3(0, 0, 0), 1.0f, grey));
   world.lights.push_back(SphereLight(Vec3(1.2f, 1.2f, 1.2f), 0.15f, Srgb(1, 1, 1) * 40.0f));
   return world.cameras.add_camera(PinholeCamera(rx, ry, 60.0f, Vec3(-0.45f, 0.2f, 2.0f) * 2.25f, Vec3(0, 0, 0), Vec3(0, 1, 0)));
@@ -84,8 +96,9 @@ int main(int argc, char** argv) {
   int max_rounds = kAdaptiveMaxRounds;
   bool res_set = false, samples_set = false, bounces_set = false;
   const char *out = nullptr, *dump = nullptr, *dump_scene = nullptr;
-  bool orbit_trap = false, panorama = false;
+  bool orbit_trap = false, panorama = false, metallic = false;
   OrbitTrapAlbedo trap{0.0f, 1.0f, Srgb(0, 0, 0), Srgb(0, 0, 0)};
+  MetalArgs metal{Srgb(0, 0, 0), 0.0f};
   for (int i = 1; i < argc; ++i) {
     if (!strcmp(argv[i], "--config") && i + 1 < argc) config = atoi(argv[++i]);
     else if (!strcmp(argv[i], "--res") && i + 2 < argc) W = atoi(argv[++i]), H = atoi(argv[++i]), res_set = true;
@@ -105,9 +118,15 @@ int main(int argc, char** argv) {
       for (int k = 0; k < 8; ++k) v[k] = (float)atof(argv[++i]);
       trap = OrbitTrapAlbedo{v[0], v[1], Srgb(v[2], v[3], v[4]), Srgb(v[5], v[6], v[7])};
       orbit_trap = true;
+    } else if (!strcmp(argv[i], "--metallic") && i + 4 < argc) {
+      float v[4];
+      for (int k = 0; k < 4; ++k) v[k] = (float)atof(argv[++i]);
+      metal = MetalArgs{Srgb(v[0], v[1], v[2]), v[3]};
+      metallic = true;
     } else {
       fprintf(stderr, "usage: rayn_host [--config 1..5] [--res W H] [--samples S] [--bounces B] [--adaptive THRESHOLD [--rounds MAX]] "
-                      "[--denoise L [--denoise-albedo] [--denoise-variance]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--panorama] [--out f.ppm] "
+                      "[--denoise L [--denoise-albedo] [--denoise-variance]] [--orbit-trap LO HI R0 G0 B0 R1 G1 B1] [--metallic R G B ROUGHNESS] "
+                      "[--panorama] [--out f.ppm] "
                       "[--dump f.bin]\n");
       return 2;
     }
@@ -130,9 +149,9 @@ int main(int argc, char** argv) {
   }
   try {
     World world;
-    CameraHandle camera = config == 1 ? setup_single_sphere(world, (float)W, (float)H)
+    CameraHandle camera = config == 1 ? setup_single_sphere(world, (float)W, (float)H, metallic ? &metal : nullptr)
                                       : setup(world, (float)W, (float)H, config == 4, config == 3 ? 0 : 1, config == 4,
-                                              orbit_trap ? &trap : nullptr);
+                                              orbit_trap ? &trap : nullptr, metallic ? &metal : nullptr);
     if (panorama) {
       const RaynCamera& c = world.cameras.get(camera);
       camera = world.cameras.add_camera(EquirectangularCamera((float)H, Vec3(c.origin[0], c.origin[1], c.origin[2]), Vec3(c.at[0], c.at[1], c.at[2]),

@@ -80,6 +80,18 @@ struct Dielectric : Material {  // material.rs:150-175
     return Dielectric(albedo, r);
   }
 };
+// A glossy conductor with coloured Fresnel (include/rayn_b200.h, RAYN_MATERIAL_METALLIC): an EXTENSION with no reference
+// counterpart.  F0 per channel in albedo, or an orbit-trap palette; the exponent remap is the Dielectric's.
+struct Metallic : Material {
+  template <class A>
+  Metallic(A f0, float roughness_exponent) {
+    pod.kind = RAYN_MATERIAL_METALLIC;
+    set_albedo(f0);
+    pod.roughness = roughness_exponent;
+  }
+  template <class A>
+  static Metallic new_remap(A f0, float roughness) { return Metallic(f0, Dielectric::new_remap(Srgb(0, 0, 0), roughness).pod.roughness); }
+};
 struct Sky : Material {  // material.rs:394-404
   Sky(Srgb top, Srgb bottom) {
     pod.kind = RAYN_MATERIAL_SKY;

@@ -123,7 +123,7 @@ class OrbitTrapAlbedo:
     by orbit trap: the smallest squared radius the distance estimator's iteration reaches at the hit point (Mandelbox: the r2
     its sphere fold divides by; Mandelbulb: |w|^2), mapped linearly from [trap_lo, trap_hi] onto albedo_lo .. albedo_hi and
     clamped.  Hits on analytic spheres take albedo_hi.  The exact statement is in include/rayn_b200.h (RaynAlbedoTrap).
-    Pass it as the albedo of Lambertian(...), Dielectric(...) or Dielectric.new_remap(...)."""
+    Pass it as the albedo of Lambertian(...), Dielectric(...) or Dielectric.new_remap(...), or as the F0 of Metallic(...)."""
 
     def __init__(self, trap_lo, trap_hi, albedo_lo, albedo_hi):
         self.trap_lo, self.trap_hi = f32(trap_lo), f32(trap_hi)
@@ -149,6 +149,12 @@ def _albedo(albedo):
     return _arr(albedo), None
 
 
+def _remap_roughness(roughness):
+    """Roughness in [0,1] -> Phong exponent, material.rs:167-174 (Dielectric::new_remap), in float32."""
+    r = f32(1.0) - f32(roughness)
+    return f32(1.0) + r * r * r * r * f32(300.0)
+
+
 class Lambertian:  # material.rs:91-100
     def __init__(self, albedo):
         self.albedo, self.albedo_gen = _albedo(albedo)
@@ -168,13 +174,38 @@ class Dielectric:  # material.rs:150-175
     @staticmethod
     def new_remap(albedo, roughness):
         """Roughness in [0,1] -> Phong exponent, material.rs:167-174."""
-        r = f32(1.0) - f32(roughness)
-        r = f32(1.0) + r * r * r * r * f32(300.0)
-        return Dielectric(albedo, r)
+        return Dielectric(albedo, _remap_roughness(roughness))
 
     def flatten(self):
         m = L.RaynMaterial()
         m.kind = L.MATERIAL_DIELECTRIC
+        m.albedo[:] = self.albedo.tolist()
+        m.roughness = float(self.roughness)
+        return m
+
+
+class Metallic:
+    """A glossy conductor with coloured Fresnel: the Dielectric's Phong specular lobe with Schlick F0 per channel and no
+    diffuse term.  An extension with no reference counterpart (rayn's material.rs carries a Metallic only as commented-out
+    code); the exact statement is in include/rayn_b200.h (RAYN_MATERIAL_METALLIC).  f0 may be an OrbitTrapAlbedo: the palette
+    then replaces F0 at every hit."""
+
+    def __init__(self, f0, roughness_exponent):
+        self.albedo, self.albedo_gen = _albedo(f0)
+        self.roughness = f32(roughness_exponent)
+
+    @property
+    def f0(self):
+        return self.albedo
+
+    @staticmethod
+    def new_remap(f0, roughness):
+        """Roughness in [0,1] -> Phong exponent, as Dielectric.new_remap."""
+        return Metallic(f0, _remap_roughness(roughness))
+
+    def flatten(self):
+        m = L.RaynMaterial()
+        m.kind = L.MATERIAL_METALLIC
         m.albedo[:] = self.albedo.tolist()
         m.roughness = float(self.roughness)
         return m
