@@ -238,7 +238,11 @@ typedef struct RaynSceneDesc {
 
 typedef enum RaynMemSpace { RAYN_MEM_HOST = 0, RAYN_MEM_DEVICE = 1 } RaynMemSpace;
 
-/* ---- one call of render_frame_into (src/film.rs:382-395) --------------------------- */
+/* ---- one call of render_frame_into (src/film.rs:382-395) ---------------------------
+ * Render limits, checked on the host before any launch; each returns RAYN_ERR_UNSUPPORTED:
+ *   spp = 4*samples <= 16384                        the film resolve stages 8 B per sample of a pixel in shared memory
+ *   tile_w*tile_h*spp + 4*n_hitables < 2^22         a path's shading slot is a 22-bit field of its film key
+ *   max_bounces <= 254                              a path's depth is an 8-bit field of its film key                      */
 typedef struct RaynFrameDesc {
   int32_t width, height;   /* Film.res                                                     */
   int32_t tile_w, tile_h;  /* tile_size; main.rs passes 16x16                              */
@@ -777,6 +781,30 @@ int32_t rayn_b200_kat_light_sample_volume(RaynContext* ctx, const RaynLight* lig
 int32_t rayn_b200_kat_bsdf(RaynContext* ctx, const RaynMaterial* mat, int64_t n, const float* normals3,
                            const float* wo3, const float* s1d, const float* u4, float* out_wi3,
                            float* out_f3, float* out_pdf, float* out_feval3);
+
+/* The film resolve of rayn_b200_render_frame (moments != NULL: of rayn_b200_render_frame_moments) over path records given by
+ * the caller, laid out as a render's pass holds them.  R = tile_w*tile_h*spp, spp = 4*samples; path
+ * k*R + (xl*th + yl)*spp + sample belongs to sample `sample` of pixel (xl, yl) of tile tile_ids[k] (th: the tile's height
+ * clipped to the image, tiles as film.rs:399-409), for k < n_tiles <= 65535:
+ *   term[]  u32  kind << 30 | depth << 22 | shading slot: kind 1 a Color sample, 2 a Background sample, 0 none
+ *   nrm0[]  4 floats per path: the depth-0 normal xyz and, as the bits of w, the depth-0 shading slot + 1 (0: none)
+ *   rad[]   4 floats per path: the radiance xyz (w unused)
+ * Per pixel, the valid records in sample order are stably sorted by nrm0.w for the normal and alpha sums, and by
+ * (depth, slot) for the colour and background sums; each sum is strictly sequential in float from +0 and divided by
+ * (float)spp, and alpha is the count of nrm0 records over spp.  Slots must be < R + 4*n_hitables and depths <= max_bounces.
+ * The non-NULL host planes (W*H pixels, as RaynFilmPlanes / RaynMomentPlanes) are copied in, written at the pixels of the
+ * given tiles and copied back.  The limits at RaynFrameDesc apply.  *out_plan receives the launch the resolve ran with,
+ * the same as a render of that geometry: the padded spp np, warps per CTA, the significant bits of a slot and of a depth
+ * that its radix sort walks (slot_bits + 1 for the normal order, slot_bits + depth_bits for the colour order), and the
+ * dynamic shared memory per CTA in bytes.                                                                                   */
+typedef struct RaynResolvePlan {
+  int32_t np, wpc, slot_bits, depth_bits;
+  int64_t smem_bytes;
+} RaynResolvePlan;
+int32_t rayn_b200_kat_resolve(RaynContext* ctx, int32_t width, int32_t height, int32_t tile_w, int32_t tile_h, int32_t samples,
+                              int32_t max_bounces, int32_t n_hitables, int32_t n_tiles, const int32_t* tile_ids, const uint32_t* term,
+                              const float* nrm0, const float* rad, const RaynFilmPlanes* planes, const RaynMomentPlanes* moments,
+                              RaynResolvePlan* out_plan);
 
 /* Which march-kernel specialisation upload_scene selected for hitable `hitable_index` of the current scene: -1 analytic sphere,
  * 0 generic Mandelbox, 1 / 2 packed Mandelbox (12 / n iterations), 3 Mandelbulb, 4 / 5 = 1 / 2 with the three-operation

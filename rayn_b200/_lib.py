@@ -120,6 +120,10 @@ class RaynAdaptiveDesc(C.Structure):
     _fields_ = [("min_rounds", i32), ("max_rounds", i32), ("threshold", f32)]
 
 
+class RaynResolvePlan(C.Structure):
+    _fields_ = [("np", i32), ("wpc", i32), ("slot_bits", i32), ("depth_bits", i32), ("smem_bytes", i64)]
+
+
 class RaynConfig(C.Structure):
     _fields_ = [("device", i32), ("max_paths_per_pass", i64), ("flags", i32)]
 
@@ -201,6 +205,8 @@ SYMBOLS = {
     "rayn_b200_kat_light_sample": (i32, [C.c_void_p, C.POINTER(RaynLight), i64, fp, fp, fp, fp, fp]),
     "rayn_b200_kat_light_sample_volume": (i32, [C.c_void_p, C.POINTER(RaynLight), i64, fp, fp, fp, fp, fp, fp]),
     "rayn_b200_kat_bsdf": (i32, [C.c_void_p, C.POINTER(RaynMaterial), i64, fp, fp, fp, fp, fp, fp, fp, fp]),
+    "rayn_b200_kat_resolve": (i32, [C.c_void_p, i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(C.c_uint32), fp, fp,
+                                    C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes), C.POINTER(RaynResolvePlan)]),
     "rayn_b200_debug_sdf_variant": (i32, [C.c_void_p, i32]),
     "rayn_b200_debug_enable_queue_log": (i32, [C.c_void_p, i32]),
     "rayn_b200_debug_read_queue_log": (i64, [C.c_void_p, C.POINTER(i32), i64]),

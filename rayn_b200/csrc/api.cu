@@ -594,11 +594,58 @@ int64_t rayn_b200_debug_read_queue_log(RaynContext* ctx, int32_t* out, int64_t c
 
 }  // extern "C"
 
+// ---- the film resolve (k_resolve): its limits and its launch plan, for render jobs and rayn_b200_kat_resolve -----------
+static int resolve_np(int spp) {  // a pixel's paths padded to a power of two >= 32: the per-warp arrays of k_resolve
+  int np = 32;
+  while (np < spp) np <<= 1;
+  return np;
+}
+
+// The render limits stated at RaynFrameDesc in include/rayn_b200.h, for tiles of tw x th pixels at spp paths per pixel.
+static int32_t resolve_limits(RaynContext* ctx, int tw, int th, int spp, int mb, int n_hit) {
+  if (mb >= TERM_MAX_DEPTH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "max_bounces = %d: the film key holds depths up to %d", mb, TERM_MAX_DEPTH - 1);
+  const int64_t R64 = (int64_t)tw * th * spp;
+  if (R64 + 4 * n_hit >= TERM_MAX_SLOTS)
+    return fail(ctx, RAYN_ERR_UNSUPPORTED, "tile_w*tile_h*spp + 4*n_hitables = %lld: not below the 2^%d slot key space", (long long)(R64 + 4 * n_hit),
+                TERM_DEPTH_SHIFT);
+  if (resolve_warps_per_cta(resolve_np(spp)) < 1)
+    return fail(ctx, RAYN_ERR_UNSUPPORTED, "spp = %d: the film resolve holds 8 B per sample of a pixel in shared memory (max 16384 spp)", spp);
+  return RAYN_OK;
+}
+
+// k_resolve's launch plan for tiles of QS shading slots at spp paths per pixel and max_bounces mb (the limits checked): the
+// padded spp, warps per CTA, the significant bits of a shading slot (< QS) and of a depth (<= mb) - what the radix sort
+// walks - and the dynamic shared memory, which it grants the instance.
+static int32_t resolve_plan(RaynContext* ctx, int spp, int QS, int mb, bool mom, RaynResolvePlan* rp) {
+  rp->np = resolve_np(spp);
+  rp->wpc = resolve_warps_per_cta(rp->np, mom);
+  if (rp->wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "spp = %d does not fit the film resolve's shared memory", spp);
+  rp->slot_bits = 5, rp->depth_bits = 1;
+  while ((1 << rp->slot_bits) < QS + 1) ++rp->slot_bits;
+  while ((1 << rp->depth_bits) < mb + 1) ++rp->depth_bits;
+  rp->smem_bytes = (int64_t)resolve_smem_per_warp(rp->np, mom) * rp->wpc;
+  CU(cudaFuncSetAttribute(mom ? k_resolve<true> : k_resolve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rp->smem_bytes));
+  return RAYN_OK;
+}
+
+// k_resolve of the pb.n_tiles tiles of a pass into the device planes dp (and, mom, the moment planes), planned by resolve_plan.
+static void resolve_launch(const RaynResolvePlan& rp, bool mom, const DevFrame& fr, const PassBufs& pb, const RaynFilmPlanes& dp, float* dm_color,
+                           float* dm_bg, cudaStream_t st) {
+  const dim3 grid((fr.tile_w * fr.tile_h + rp.wpc - 1) / rp.wpc, pb.n_tiles);
+  const unsigned threads = rp.wpc * 32;
+  const size_t smem = (size_t)rp.smem_bytes;
+  if (mom)
+    k_resolve<true><<<grid, threads, smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, rp.np, rp.wpc, rp.slot_bits, rp.depth_bits,
+                                                 dm_color, dm_bg);
+  else
+    k_resolve<false><<<grid, threads, smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, rp.np, rp.wpc, rp.slot_bits, rp.depth_bits);
+}
+
 // ---- the stages a render and the albedo pass (rayn_b200_render_albedo) share ----------------------------------------
 // What a render derives from its frame (frame_check) and from the uploaded scene (scene_plan) before it launches anything.
 struct FramePlan {
   DevFrame fr;
-  int R, QS, np, wpc;  // paths and shading slots per tile; k_resolve's padded spp and warps per CTA
+  int R, QS;  // paths and shading slots per tile
   bool simple, traps, metal, fold_all, volume_on;
   int fold_pre, n_fold, ns, seg_per_path, lc_ns;
 };
@@ -638,17 +685,9 @@ static int32_t frame_check(RaynContext* ctx, const RaynFrameDesc* f, bool tiles_
   const int stride = f->tile_stride > 0 ? f->tile_stride : 1;
   if (!tiles_given && !f->tile_list && (f->tile_offset < 0 || f->tile_offset >= stride))
     return fail(ctx, RAYN_ERR_INVALID_ARG, "tile_offset %d not in [0,%d)", f->tile_offset, stride);
-  if (mb >= TERM_MAX_DEPTH) return fail(ctx, RAYN_ERR_UNSUPPORTED, "max_bounces > %d", TERM_MAX_DEPTH - 1);
-  const int64_t R64 = (int64_t)f->tile_w * f->tile_h * spp;
-  const int n_hit = ctx->scene.n_hit;
-  if (R64 + 4 * n_hit >= TERM_MAX_SLOTS)
-    return fail(ctx, RAYN_ERR_UNSUPPORTED, "tile_w*tile_h*spp = %lld exceeds the 2^%d slot key space", (long long)R64, TERM_DEPTH_SHIFT);
-  int& np = P->np;
-  np = 32;
-  while (np < spp) np <<= 1;
-  const int wpc = P->wpc = resolve_warps_per_cta(np);
-  if (wpc < 1 || np > 65536) return fail(ctx, RAYN_ERR_UNSUPPORTED, "spp = %d: the film resolve holds 6 B per sample of a pixel in shared memory (max 32768 spp)", spp);
-  P->R = (int)R64, P->QS = P->R + 4 * n_hit;
+  int32_t rc = resolve_limits(ctx, f->tile_w, f->tile_h, spp, mb, ctx->scene.n_hit);
+  if (rc) return rc;
+  P->R = f->tile_w * f->tile_h * spp, P->QS = P->R + 4 * ctx->scene.n_hit;
   CU(cudaSetDevice(ctx->device));
   {  // a previous call that failed half way through a graph capture must not leave the stream capturing
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -932,11 +971,12 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   PassBufs& pb = J.pb;
   const std::vector<int>& my_tiles = ctx->job_tiles;
   const bool mom = moments != nullptr;
-  const int mb = fr.max_bounces, np = P.np, wpc = mom ? resolve_warps_per_cta(np, true) : P.wpc, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
+  const int mb = fr.max_bounces, R = P.R, QS = P.QS, n_hit = ctx->scene.n_hit, n_sdf = ctx->scene.n_sdf, n_fold = P.n_fold;
   const int* sdf_idx = ctx->scene.sdf_idx;
   const bool simple = P.simple, motion = ctx->scene.sph_moving != 0, traps = P.traps, metal = P.metal, volume_on = P.volume_on;
 
-  if (mom && wpc < 1) return fail(ctx, RAYN_ERR_UNSUPPORTED, "render_frame_moments: spp = %d does not fit the film resolve's shared memory", fr.spp);
+  RaynResolvePlan rp;
+  if ((rc = resolve_plan(ctx, fr.spp, QS, mb, mom, &rp))) return rc;
   const size_t npx = (size_t)f->width * f->height;
   RaynFilmPlanes dp = *out;  // the device-space planes the film is rendered into
   float *dm_color = mom ? moments->color_lum2 : nullptr, *dm_bg = mom ? moments->background_lum2 : nullptr;  // ... and moment planes
@@ -958,12 +998,6 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
   dp.space = RAYN_MEM_DEVICE;
   if (dev_planes_out) *dev_planes_out = dp;
 
-  const size_t res_smem = resolve_smem_per_warp(np, mom) * wpc;
-  int slot_bits = 5, depth_bits = 1;  // significant bits of a shading slot (< QS) and of a depth (<= max_bounces): what k_resolve's radix sort walks
-  while ((1 << slot_bits) < QS + 1) ++slot_bits;
-  while ((1 << depth_bits) < mb + 1) ++depth_bits;
-  CU(cudaFuncSetAttribute(mom ? k_resolve<true> : k_resolve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)res_smem));
-
   // Small single-pass frames are launch bound (config 1: ~20 launches of a few microseconds each): capture the whole kernel
   // sequence of the pass once and replay it as ONE graph launch while nothing that is baked into the launches changes
   // (scene, frame geometry, every pointer, the tile set).
@@ -983,7 +1017,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
     // grows, so a graph is replayed only into the staging it was captured with
     float* planes6[6] = {dp.color, dp.alpha, dp.background, dp.normal, dm_color, dm_bg};
     key = fnv1a(key, planes6, sizeof planes6);
-    const int misc[7] = {np, wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0, mom ? 1 : 0};  // mom: the k_resolve instance
+    const int misc[7] = {rp.np, rp.wpc, mb, n_fold, simple ? 1 : 0, motion ? 1 : 0, mom ? 1 : 0};  // mom: the k_resolve instance
     key = fnv1a(key, misc, sizeof misc);
     key = fnv1a(key, my_tiles.data(), my_tiles.size() * sizeof(int));
     if (ctx->graph_exec && ctx->graph_key == key) {
@@ -1110,12 +1144,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
       }
     }
     timed_begin(ctx, RAYN_K_RESOLVE);
-    if (mom)
-      k_resolve<true><<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc,
-                                                                                                     slot_bits, depth_bits, dm_color, dm_bg);
-    else
-      k_resolve<false><<<dim3((f->tile_w * f->tile_h + wpc - 1) / wpc, nt), wpc * 32, res_smem, st>>>(fr, pb, dp.color, dp.alpha, dp.background, dp.normal, np, wpc,
-                                                                                                      slot_bits, depth_bits);
+    resolve_launch(rp, mom, fr, pb, dp, dm_color, dm_bg, st);
     timed_end(ctx, RAYN_K_RESOLVE);
     if (capturing) {
       cudaGraph_t graph = nullptr;
@@ -2265,3 +2294,49 @@ int32_t rayn_b200_kat_bsdf(RaynContext* ctx, const RaynMaterial* mat, int64_t n,
 }
 
 }  // extern "C"
+
+// The film resolve of render jobs (resolve_plan, resolve_launch) over path records given by the caller.
+extern "C" int32_t rayn_b200_kat_resolve(RaynContext* ctx, int32_t width, int32_t height, int32_t tile_w, int32_t tile_h, int32_t samples,
+                                         int32_t max_bounces, int32_t n_hitables, int32_t n_tiles, const int32_t* tile_ids, const uint32_t* term,
+                                         const float* nrm0, const float* rad, const RaynFilmPlanes* planes, const RaynMomentPlanes* moments,
+                                         RaynResolvePlan* out_plan) {
+  if (!ctx) return fail(nullptr, RAYN_ERR_INVALID_ARG, "ctx is NULL");
+  if (!tile_ids || !term || !nrm0 || !rad || !planes || !out_plan) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_resolve: NULL");
+  if (planes->space != RAYN_MEM_HOST || (moments && moments->space != RAYN_MEM_HOST)) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_resolve: planes must be host memory");
+  if (width <= 0 || height <= 0 || tile_w <= 0 || tile_h <= 0 || samples <= 0 || max_bounces < 0 || n_hitables < 0 ||
+      n_hitables > RAYN_MAX_HITABLES || n_tiles <= 0 || n_tiles > 65535)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_resolve: bad geometry");
+  const int spp = 4 * samples;
+  int32_t rc = resolve_limits(ctx, tile_w, tile_h, spp, max_bounces, n_hitables);
+  if (rc) return rc;
+  DevFrame fr{};
+  fr.W = width, fr.H = height, fr.tile_w = tile_w, fr.tile_h = tile_h, fr.samples = samples, fr.spp = spp, fr.max_bounces = max_bounces, fr.vm = 2;
+  tile_grid_of(width, height, tile_w, tile_h, &fr.ntx, &fr.nty);
+  for (int i = 0; i < n_tiles; ++i)
+    if (tile_ids[i] < 0 || tile_ids[i] >= fr.ntx * fr.nty) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_resolve: tile id %d not in [0,%d)", tile_ids[i], fr.ntx * fr.nty);
+  CU(cudaSetDevice(ctx->device));
+  const bool mom = moments != nullptr;
+  PassBufs pb{};
+  pb.n_tiles = n_tiles, pb.R = tile_w * tile_h * spp, pb.QS = pb.R + 4 * n_hitables;
+  if ((rc = resolve_plan(ctx, spp, pb.QS, max_bounces, mom, out_plan))) return rc;
+  const size_t paths = (size_t)n_tiles * pb.R, npx = (size_t)width * height;
+  DevTmp tmp;
+  cudaError_t e = cudaSuccess;
+  pb.tile_ids = tmp.up(tile_ids, n_tiles, &e);
+  pb.term = tmp.up(term, paths, &e);
+  pb.nrm0 = reinterpret_cast<float4*>(tmp.up(nrm0, 4 * paths, &e));
+  pb.rad = reinterpret_cast<float4*>(tmp.up(rad, 4 * paths, &e));
+  // the planes start as the caller's, so that whatever the resolve does not write comes back unchanged
+  float* const user[6] = {planes->color, planes->alpha, planes->background, planes->normal, mom ? moments->color_lum2 : nullptr,
+                          mom ? moments->background_lum2 : nullptr};
+  const int nc[6] = {3, 1, 3, 3, 1, 1};
+  float* dev[6];
+  for (int i = 0; i < 6; ++i) dev[i] = user[i] ? tmp.up(user[i], nc[i] * npx, &e) : nullptr;
+  CU(e);
+  resolve_launch(*out_plan, mom, fr, pb, RaynFilmPlanes{dev[0], dev[1], dev[2], dev[3], RAYN_MEM_DEVICE}, dev[4], dev[5], ctx->stream);
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < 6; ++i)
+    if (user[i]) CU(cudaMemcpy(user[i], dev[i], nc[i] * npx * sizeof(float), cudaMemcpyDeviceToHost));
+  return RAYN_OK;
+}

@@ -507,6 +507,22 @@ class Renderer:
                                              _fptr(pdf), _fptr(fe)), self._ctx)
         return wi, f, pdf, fe
 
+    def kat_resolve(self, width, height, tile_size, samples, max_bounces, n_hitables, tile_ids, term, nrm0, rad, planes, moments=None):
+        """The film resolve over given path records (include/rayn_b200.h: rayn_b200_kat_resolve).  term uint32 [n_tiles * R],
+        nrm0 and rad float32 [n_tiles * R, 4]; planes: flat float32 arrays keyed by CHANNELS (absent keys are not written),
+        moments: None, or float32 [2, W*H] (color_lum2, background_lum2) for the moments instance.  The arrays are updated in
+        place.  Returns the RaynResolvePlan the resolve ran with."""
+        ids = np.ascontiguousarray(tile_ids, np.int32)
+        term = np.ascontiguousarray(term, np.uint32)
+        nrm0, rad = np.ascontiguousarray(nrm0, np.float32), np.ascontiguousarray(rad, np.float32)
+        p = L.RaynFilmPlanes(*(planes[k].ctypes.data if k in planes else None for k in CHANNELS), L.MEM_HOST)
+        mp = None if moments is None else C.byref(L.RaynMomentPlanes(moments[0].ctypes.data, moments[1].ctypes.data, L.MEM_HOST))
+        plan = L.RaynResolvePlan()
+        L.check(self._lib.rayn_b200_kat_resolve(self._ctx, width, height, tile_size[0], tile_size[1], samples, max_bounces, n_hitables, len(ids),
+                                                ids.ctypes.data_as(C.POINTER(C.c_int32)), term.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                _fptr(nrm0), _fptr(rad), C.byref(p), mp, C.byref(plan)), self._ctx)
+        return plan
+
     def sdf_variant(self, hitable_index):
         """march-kernel specialisation upload_scene selected for a hitable (include/rayn_b200.h: rayn_b200_debug_sdf_variant)"""
         return int(self._lib.rayn_b200_debug_sdf_variant(self._ctx, hitable_index))

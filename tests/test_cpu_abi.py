@@ -55,7 +55,7 @@ def test_all_library_variants_load_and_export_the_abi():
 def test_struct_layouts_match_the_c_compiler(tmp_path):
     from rayn_b200 import _lib as L
     names = ["RaynHitable", "RaynMaterial", "RaynLight", "RaynCamera", "RaynVolume", "RaynRenderConsts", "RaynSceneDesc",
-             "RaynFrameDesc", "RaynFilmPlanes", "RaynConfig", "RaynStats"]
+             "RaynFrameDesc", "RaynFilmPlanes", "RaynConfig", "RaynStats", "RaynResolvePlan"]
     src = tmp_path / "sz.c"
     src.write_text('#include <stdio.h>\n#include "rayn_b200.h"\nint main(){' +
                    "".join(f'printf("{n} %zu\\n", sizeof({n}));' for n in names) +
