@@ -806,6 +806,33 @@ int32_t rayn_b200_kat_resolve(RaynContext* ctx, int32_t width, int32_t height, i
                               const float* nrm0, const float* rad, const RaynFilmPlanes* planes, const RaynMomentPlanes* moments,
                               RaynResolvePlan* out_plan);
 
+/* The persistent march kernels of render_frame over data given by the caller, laid out as a render's pass holds it, through
+ * the launch helpers a render uses (grids from the SDF's specialisation, rayn_b200_debug_sdf_variant, and the resident wave;
+ * paired != 0: the half wave of a pass that runs beside another).  Each runs on the uploaded scene and its render constants,
+ * in buffers of its own: the context's stats are not touched.  *out_evals receives the kernel's distance evaluations, as
+ * RaynStats counts them.  Every index is checked before a launch (RAYN_ERR_INVALID_ARG); words the input does not name come
+ * back unchanged.
+ *
+ * k_extend_march, TracedSDF::hit (sdf.rs:59-83) of SDF hitable hk with the threshold closure of `depth` (film.rs:540-551)
+ * over n_tiles <= 65535 tiles of R paths (n_tiles*R < 2^31): path k*R + id has o_time[] (origin.xyz, time) and d_t[] (dir.xyz,
+ * closest t so far) and q_key[] (hitable of that t, -1 none); tile k's live paths are q_live[k*R + i] < R for i < n_live[k] <= R.
+ * A march ending at t < d_t.w, or (spheres_first != 0) at t == d_t.w with q_key > hk, writes d_t.w = t and q_key = hk.       */
+int32_t rayn_b200_kat_march_extend(RaynContext* ctx, int32_t hk, int32_t depth, int32_t spheres_first, int32_t paired, int32_t n_tiles,
+                                   int32_t R, const int32_t* n_live, const int32_t* q_live, const float* o_time, float* d_t,
+                                   int32_t* q_key, int64_t* out_evals);
+/* k_shadow, TracedSDF::occluded (sdf.rs:25-57) of SDF ordinal j over the queue of n_seg < 2^30 segments: seg_a[] (start.xyz,
+ * max_dist), seg_b[] (unit dir.xyz, bits of owner << 4 | bit, owner < n_vis <= 2^27).  An occluded segment clears bit `bit` of
+ * vis[owner].                                                                                                                */
+int32_t rayn_b200_kat_march_shadow(RaynContext* ctx, int32_t j, int32_t paired, int64_t n_seg, const float* seg_a, const float* seg_b,
+                                   int64_t n_vis, uint32_t* vis, int64_t* out_evals);
+/* k_normals, get_shading_info (sdf.rs:85-101) of SDF ordinal j at `depth` over n_tiles <= 65535 tiles of R paths and QS >= R
+ * shading slots: bin_start[k*(n_hitables + 1) + o] is the first slot of hitable o's bin in tile k (ascending, <= QS, the last
+ * entry the end of the queue), q_shade[k*QS + s] a path id < R, or < 0 for a padding lane.  Path g of SDF j's bin gets
+ * nrm[g] = (normal.xyz, offset_by) and, if the hitable's material has an orbit trap, trap_s[g] (else trap_s may be NULL).     */
+int32_t rayn_b200_kat_march_normals(RaynContext* ctx, int32_t j, int32_t depth, int32_t n_tiles, int32_t R, int32_t QS, const int32_t* bin_start,
+                                    const int32_t* q_shade, const float* o_time, const float* d_t, float* nrm, float* trap_s,
+                                    int64_t* out_evals);
+
 /* Which march-kernel specialisation upload_scene selected for hitable `hitable_index` of the current scene: -1 analytic sphere,
  * 0 generic Mandelbox, 1 / 2 packed Mandelbox (12 / n iterations), 3 Mandelbulb, 4 / 5 = 1 / 2 with the three-operation
  * sphere-fold division, which upload_scene selects only after dividing by EVERY float in [min_rad_sq, fixed_rad_sq] on this

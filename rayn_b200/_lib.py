@@ -207,6 +207,10 @@ SYMBOLS = {
     "rayn_b200_kat_bsdf": (i32, [C.c_void_p, C.POINTER(RaynMaterial), i64, fp, fp, fp, fp, fp, fp, fp, fp]),
     "rayn_b200_kat_resolve": (i32, [C.c_void_p, i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(C.c_uint32), fp, fp,
                                     C.POINTER(RaynFilmPlanes), C.POINTER(RaynMomentPlanes), C.POINTER(RaynResolvePlan)]),
+    "rayn_b200_kat_march_extend": (i32, [C.c_void_p, i32, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), fp, fp, C.POINTER(i32),
+                                         C.POINTER(i64)]),
+    "rayn_b200_kat_march_shadow": (i32, [C.c_void_p, i32, i32, i64, fp, fp, i64, C.POINTER(C.c_uint32), C.POINTER(i64)]),
+    "rayn_b200_kat_march_normals": (i32, [C.c_void_p, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), fp, fp, fp, fp, C.POINTER(i64)]),
     "rayn_b200_debug_sdf_variant": (i32, [C.c_void_p, i32]),
     "rayn_b200_debug_enable_queue_log": (i32, [C.c_void_p, i32]),
     "rayn_b200_debug_read_queue_log": (i64, [C.c_void_p, C.POINTER(i32), i64]),

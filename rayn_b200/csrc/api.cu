@@ -825,6 +825,39 @@ static unsigned march_grid(const RaynContext* ctx, const Job& J, int occ) {
   return (unsigned)ctx->n_sm * (J.paired ? (occ + 1) / 2 : occ);
 }
 
+// ---- the launches of the march kernels, shared by render jobs and the known-answer hooks (rayn_b200_kat_march_*) --------
+// k_scan_live: the 128-ray batches of the pass's live rays (J.batch_prefix) and zeroed work counters, before a depth's
+// closest-hit stage.
+static void scan_live_launch(const Job& J) { k_scan_live<<<1, SCAN_T, 0, J.st>>>(J.pb, J.batch_prefix, J.work_ctr); }
+
+// k_extend_march of SDF hitable hk over the batches of scan_live_launch; sf: the spheres were folded in first (fold_all).
+static void extend_march_launch(const RaynContext* ctx, const Job& J, const Thr& thr, int hk, int sf) {
+  const int v = ctx->sdf_var[hk];
+  if (thr.is_const)
+    DISPATCH_SDFV(v, (k_extend_march<V, true><<<march_grid(ctx, J, ctx->occ_ext[1][v]), EXT_T, 0, J.st>>>(ctx->scene, J.pb, thr, hk, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
+  else
+    DISPATCH_SDFV(v, (k_extend_march<V, false><<<march_grid(ctx, J, ctx->occ_ext[0][v]), EXT_T, 0, J.st>>>(ctx->scene, J.pb, thr, hk, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
+}
+
+// k_shadow over the segment queue of SDF ordinal j.
+static void shadow_launch(const RaynContext* ctx, const Job& J, int j) {
+  const int hk = ctx->scene.sdf_idx[j], v = ctx->sdf_var[hk];
+  DISPATCH_SDFV(v, (k_shadow<V><<<march_grid(ctx, J, ctx->occ_shd[v]), SHD_T, 0, J.st>>>(ctx->scene, J.pb, hk, j, J.work_ctr + WC_SHADOW + j)));
+}
+
+// k_scan_slots: the work lists of the slot-parallel kernels, once the shading queues of a depth are binned.
+static void scan_slots_launch(const RaynContext* ctx, const Job& J) { k_scan_slots<<<1, SCAN_T, 0, J.st>>>(ctx->scene, J.pb); }
+
+// k_normals over the bin of SDF ordinal j (work list of scan_slots_launch); the TRAP instance when the hitable's material has
+// an orbit-trap albedo.
+static void normals_launch(const RaynContext* ctx, const Job& J, const Thr& thr, int j) {
+  const int hk = ctx->scene.sdf_idx[j], v = ctx->sdf_var[hk];
+  if ((ctx->scene.trap_mask >> ctx->scene.hit[hk].material) & 1u)
+    DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx, J, ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, J.st>>>(ctx->scene, J.pb, thr, hk, j, J.work_ctr + WC_NORMALS + j)))
+  else
+    DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx, J, ctx->occ_nrm[v]), SLOT_BLOCK, 0, J.st>>>(ctx->scene, J.pb, thr, hk, j, J.work_ctr + WC_NORMALS + j)))
+}
+
 // One depth's closest-hit stage (the non-legacy kernels): k_scan_live, then the fold over the live rays of the pass.
 static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
   cudaStream_t st = J.st;
@@ -833,7 +866,7 @@ static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
   const bool fold_all = J.P.fold_all, motion = ctx->scene.sph_moving != 0;
   const unsigned sph_grid = resident(ctx, J, ctx->occ_sph);
   timed_begin(ctx, RAYN_K_MISC);
-  k_scan_live<<<1, SCAN_T, 0, st>>>(pb, J.batch_prefix, J.work_ctr);
+  scan_live_launch(J);
   timed_end(ctx, RAYN_K_MISC);
   // fold order of hitable.rs:177-198: runs of spheres as coherent kernels, each SDF as a persistent march.  The
   // spheres before the first SDF were already folded in by the kernel that produced the rays (fold_pre >= 0).
@@ -849,13 +882,8 @@ static int32_t extend_enqueue(RaynContext* ctx, const Job& J, const Thr& thr) {
     }
     if (e < n_hit) {
       if (n_march++ > 0) CU(cudaMemsetAsync(J.work_ctr + WC_EXTEND, 0, sizeof(int), st));
-      const int v = ctx->sdf_var[e];
       timed_begin(ctx, RAYN_K_EXTEND);
-      const int sf = fold_all ? 1 : 0;
-      if (thr.is_const)
-        DISPATCH_SDFV(v, (k_extend_march<V, true><<<march_grid(ctx, J, ctx->occ_ext[1][v]), EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
-      else
-        DISPATCH_SDFV(v, (k_extend_march<V, false><<<march_grid(ctx, J, ctx->occ_ext[0][v]), EXT_T, 0, st>>>(ctx->scene, pb, thr, e, sf, J.batch_prefix, J.work_ctr + WC_EXTEND)))
+      extend_march_launch(ctx, J, thr, e, fold_all ? 1 : 0);
       timed_end(ctx, RAYN_K_EXTEND);
       ++e;
     }
@@ -1072,7 +1100,7 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
       timed_begin(ctx, RAYN_K_BIN);
       k_bin_count<<<dim3(nseg, nt), BIN_T, 0, st>>>(pb, n_hit, nseg);
       k_bin_scatter<<<dim3(nseg, nt), BIN_T, 0, st>>>(pb, n_hit, nseg);
-      if (!simple) k_scan_slots<<<1, SCAN_T, 0, st>>>(ctx->scene, pb);  // work lists of k_normals / k_shade_pre / k_shade_post
+      if (!simple) scan_slots_launch(ctx, J);  // work lists of k_normals / k_shade_pre / k_shade_post
       timed_end(ctx, RAYN_K_BIN, simple ? 2 : 3);
       if (ctx->qlog_enabled) {
         h_nslots.resize(nt);
@@ -1093,12 +1121,8 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
           const RaynHitable& h = ctx->scene.hit[sdf_idx[j]];
           const int mk = ctx->scene.mat[h.material].kind;
           if (!(mk == RAYN_MATERIAL_LAMBERTIAN || mk == RAYN_MATERIAL_DIELECTRIC || mk == RAYN_MATERIAL_METALLIC || volume_on)) continue;
-          const int v = ctx->sdf_var[sdf_idx[j]];
           timed_begin(ctx, RAYN_K_NORMALS);
-          if ((ctx->scene.trap_mask >> h.material) & 1u)  // the bin's material has an orbit-trap albedo: normals + trap
-            DISPATCH_SDFV(v, (k_normals<V, true><<<resident(ctx, J, ctx->occ_nrm_trap[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, J.work_ctr + WC_NORMALS + j)))
-          else
-            DISPATCH_SDFV(v, (k_normals<V, false><<<resident(ctx, J, ctx->occ_nrm[v]), SLOT_BLOCK, 0, st>>>(ctx->scene, pb, thr, sdf_idx[j], j, J.work_ctr + WC_NORMALS + j)))
+          normals_launch(ctx, J, thr, j);
           timed_end(ctx, RAYN_K_NORMALS);
         }
         timed_begin(ctx, RAYN_K_SHADE_PRE);
@@ -1113,9 +1137,8 @@ static int32_t render_enqueue(RaynContext* ctx, const RaynFrameDesc* f, const Ra
         timed_end(ctx, RAYN_K_SHADE_PRE);
         if (ctx->scene.n_lights > 0) {
           for (int j = 0; j < n_sdf; ++j) {
-            const int v = ctx->sdf_var[sdf_idx[j]];
             timed_begin(ctx, RAYN_K_SHADOW);
-            DISPATCH_SDFV(v, (k_shadow<V><<<march_grid(ctx, J, ctx->occ_shd[v]), SHD_T, 0, st>>>(ctx->scene, pb, sdf_idx[j], j, J.work_ctr + WC_SHADOW + j)));
+            shadow_launch(ctx, J, j);
             timed_end(ctx, RAYN_K_SHADOW);
           }
         }
@@ -2338,5 +2361,163 @@ extern "C" int32_t rayn_b200_kat_resolve(RaynContext* ctx, int32_t width, int32_
   CU(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < 6; ++i)
     if (user[i]) CU(cudaMemcpy(user[i], dev[i], nc[i] * npx * sizeof(float), cudaMemcpyDeviceToHost));
+  return RAYN_OK;
+}
+
+// ---- the persistent march kernels over rays, segments and shading bins given by the caller ------------------------------
+// Each hook lays the caller's data out as a pass holds it, in buffers of its own (the context's pass sets and stats are not
+// touched), and runs the launch helper of render jobs.  Its own counters return the kernel's distance evaluations.
+struct KatMarch {
+  DevTmp tmp;
+  Job J{};
+  unsigned long long* counters = nullptr;
+};
+// (after job_ready)
+static int32_t kat_march_begin(RaynContext* ctx, const char* call, int hk, int paired, int n_tiles, int R, int QS, KatMarch* K) {
+  if (hk < 0 || hk >= ctx->scene.n_hit || ctx->scene.hit[hk].kind == RAYN_HITABLE_SPHERE) return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: hitable %d is not an SDF", call, hk);
+  if (n_tiles < 1 || n_tiles > 65535 || R < 1 || QS < R || (int64_t)n_tiles * QS > INT_MAX)
+    return fail(ctx, RAYN_ERR_INVALID_ARG, "%s: %d tiles of %d paths and %d slots: need 1 <= tiles <= 65535, R >= 1, QS >= R, tiles*QS < 2^31", call, n_tiles,
+                R, QS);
+  CU(cudaSetDevice(ctx->device));
+  Job& J = K->J;
+  J.P.R = R, J.P.QS = QS;
+  J.pb.n_tiles = n_tiles, J.pb.R = R, J.pb.QS = QS;
+  J.paired = paired != 0;
+  J.st = ctx->stream;
+  cudaError_t e = cudaSuccess;
+  J.batch_prefix = K->tmp.up<int>(nullptr, (size_t)n_tiles + 1, &e);
+  J.work_ctr = K->tmp.up<int>(nullptr, WC_TOTAL, &e);
+  K->counters = J.pb.counters = K->tmp.up<unsigned long long>(nullptr, CNT_TOTAL, &e);
+  CU(e);
+  CU(cudaMemsetAsync(J.work_ctr, 0, WC_TOTAL * sizeof(int), J.st));
+  CU(cudaMemsetAsync(J.pb.counters, 0, CNT_TOTAL * sizeof(unsigned long long), J.st));
+  CU(cudaStreamSynchronize(J.st));  // before the caller's data is copied in on the legacy stream
+  return RAYN_OK;
+}
+static int32_t kat_march_end(RaynContext* ctx, const KatMarch& K, int counter, int64_t* out_evals) {
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(ctx->stream));
+  unsigned long long c = 0;
+  CU(cudaMemcpy(&c, K.counters + counter, sizeof c, cudaMemcpyDeviceToHost));
+  *out_evals = (int64_t)c;
+  return RAYN_OK;
+}
+
+extern "C" int32_t rayn_b200_kat_march_extend(RaynContext* ctx, int32_t hk, int32_t depth, int32_t spheres_first, int32_t paired, int32_t n_tiles,
+                                              int32_t R, const int32_t* n_live, const int32_t* q_live, const float* o_time, float* d_t,
+                                              int32_t* q_key, int64_t* out_evals) {
+  int32_t rc = job_ready(ctx, "kat_march_extend");
+  if (rc) return rc;
+  if (!n_live || !q_live || !o_time || !d_t || !q_key || !out_evals) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_extend: NULL");
+  if (depth < 0 || depth >= TERM_MAX_DEPTH) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_extend: depth %d not in [0,%d)", depth, TERM_MAX_DEPTH);
+  KatMarch K;
+  rc = kat_march_begin(ctx, "kat_march_extend", hk, paired, n_tiles, R, R, &K);
+  if (rc) return rc;
+  for (int t = 0; t < n_tiles; ++t) {
+    if (n_live[t] < 0 || n_live[t] > R) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_extend: n_live[%d] = %d not in [0,%d]", t, n_live[t], R);
+    for (int i = 0; i < n_live[t]; ++i) {
+      const int id = q_live[(size_t)t * R + i];
+      if (id < 0 || id >= R) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_extend: q_live[%d] of tile %d = %d not in [0,%d)", i, t, id, R);
+    }
+  }
+  PassBufs& pb = K.J.pb;
+  const size_t paths = (size_t)n_tiles * R;
+  cudaError_t e = cudaSuccess;
+  pb.n_live = K.tmp.up(n_live, n_tiles, &e);
+  pb.q_live = K.tmp.up(q_live, paths, &e);
+  pb.q_key = K.tmp.up(q_key, paths, &e);
+  pb.o_time = reinterpret_cast<float4*>(K.tmp.up(o_time, 4 * paths, &e));
+  pb.d_t = reinterpret_cast<float4*>(K.tmp.up(d_t, 4 * paths, &e));
+  CU(e);
+  scan_live_launch(K.J);
+  extend_march_launch(ctx, K.J, make_thr(ctx->scene.cam, depth), hk, spheres_first ? 1 : 0);
+  if ((rc = kat_march_end(ctx, K, CNT_EVALS_EXTEND, out_evals))) return rc;
+  CU(cudaMemcpy(d_t, pb.d_t, 4 * paths * sizeof(float), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(q_key, pb.q_key, paths * sizeof(int), cudaMemcpyDeviceToHost));
+  return RAYN_OK;
+}
+
+extern "C" int32_t rayn_b200_kat_march_shadow(RaynContext* ctx, int32_t j, int32_t paired, int64_t n_seg, const float* seg_a, const float* seg_b,
+                                              int64_t n_vis, uint32_t* vis, int64_t* out_evals) {
+  int32_t rc = job_ready(ctx, "kat_march_shadow");
+  if (rc) return rc;
+  if ((n_seg > 0 && (!seg_a || !seg_b)) || !vis || !out_evals) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: NULL");
+  if (j < 0 || j >= ctx->scene.n_sdf) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: SDF ordinal %d not in [0,%d)", j, ctx->scene.n_sdf);
+  if (n_seg < 0 || n_seg > INT_MAX / 2) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: n_seg = %lld not in [0,2^30)", (long long)n_seg);
+  if (n_vis < 1 || n_vis > ((int64_t)1 << 27)) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: n_vis = %lld not in [1,2^27]", (long long)n_vis);
+  // seg_b.w holds the bits of owner path g << 4 | light-sample bit, so bit < 16; a g above 2^27 - 1 would set the sign bit
+  for (int64_t i = 0; i < n_seg; ++i) {
+    uint32_t w;
+    memcpy(&w, seg_b + 4 * i + 3, sizeof w);
+    if (w >> 31) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: segment %lld: owner %u above 2^27 - 1", (long long)i, w >> 4);
+    if ((int64_t)(w >> 4) >= n_vis) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_shadow: segment %lld: owner %u not below n_vis", (long long)i, w >> 4);
+  }
+  KatMarch K;
+  if ((rc = kat_march_begin(ctx, "kat_march_shadow", ctx->scene.sdf_idx[j], paired, 1, 1, 1, &K))) return rc;
+  PassBufs& pb = K.J.pb;
+  cudaError_t e = cudaSuccess;
+  // queue j of a pass: entries [j * seg_cap, j * seg_cap + seg_count[j])
+  pb.seg_cap = std::max<int64_t>(n_seg, 1);
+  pb.seg_a = reinterpret_cast<float4*>(K.tmp.up<float>(nullptr, 4 * (size_t)pb.seg_cap * (j + 1), &e));
+  pb.seg_b = reinterpret_cast<float4*>(K.tmp.up<float>(nullptr, 4 * (size_t)pb.seg_cap * (j + 1), &e));
+  pb.vis = K.tmp.up(vis, (size_t)n_vis, &e);
+  CU(e);
+  pb.seg_count = K.J.work_ctr + WC_SEG_COUNT;
+  const int ns = (int)n_seg;
+  CU(cudaMemcpy(pb.seg_count + j, &ns, sizeof ns, cudaMemcpyHostToDevice));
+  if (n_seg > 0) {
+    CU(cudaMemcpy(pb.seg_a + (size_t)j * pb.seg_cap, seg_a, 16 * (size_t)n_seg, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(pb.seg_b + (size_t)j * pb.seg_cap, seg_b, 16 * (size_t)n_seg, cudaMemcpyHostToDevice));
+  }
+  CU(cudaDeviceSynchronize());  // the pageable copies above and the non-blocking stream do not order
+  shadow_launch(ctx, K.J, j);
+  if ((rc = kat_march_end(ctx, K, CNT_EVALS_SHADOW, out_evals))) return rc;
+  CU(cudaMemcpy(vis, pb.vis, (size_t)n_vis * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return RAYN_OK;
+}
+
+extern "C" int32_t rayn_b200_kat_march_normals(RaynContext* ctx, int32_t j, int32_t depth, int32_t n_tiles, int32_t R, int32_t QS,
+                                               const int32_t* bin_start, const int32_t* q_shade, const float* o_time, const float* d_t,
+                                               float* nrm, float* trap_s, int64_t* out_evals) {
+  int32_t rc = job_ready(ctx, "kat_march_normals");
+  if (rc) return rc;
+  if (!bin_start || !q_shade || !o_time || !d_t || !nrm || !out_evals) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: NULL");
+  if (j < 0 || j >= ctx->scene.n_sdf) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: SDF ordinal %d not in [0,%d)", j, ctx->scene.n_sdf);
+  if (depth < 0 || depth >= TERM_MAX_DEPTH) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: depth %d not in [0,%d)", depth, TERM_MAX_DEPTH);
+  const int hk = ctx->scene.sdf_idx[j], n_hit = ctx->scene.n_hit;
+  const bool trap = (ctx->scene.trap_mask >> ctx->scene.hit[hk].material) & 1u;
+  if (trap && !trap_s) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: the material has an orbit trap: trap_s is NULL");
+  KatMarch K;
+  if ((rc = kat_march_begin(ctx, "kat_march_normals", hk, 0, n_tiles, R, QS, &K))) return rc;
+  std::vector<int> bs((size_t)n_tiles * (RAYN_MAX_HITABLES + 1), 0), n_slots(n_tiles);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int32_t* b = bin_start + (size_t)t * (n_hit + 1);
+    for (int o = 0; o <= n_hit; ++o) {
+      if (b[o] < (o ? b[o - 1] : 0) || b[o] > QS)
+        return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: bin_start of tile %d is not ascending in [0,%d]", t, QS);
+      bs[(size_t)t * (RAYN_MAX_HITABLES + 1) + o] = b[o];
+    }
+    n_slots[t] = b[n_hit];
+    for (int s = b[hk]; s < b[hk + 1]; ++s)
+      if (q_shade[(size_t)t * QS + s] >= R) return fail(ctx, RAYN_ERR_INVALID_ARG, "kat_march_normals: slot %d of tile %d holds path %d, not below %d", s, t, q_shade[(size_t)t * QS + s], R);
+  }
+  PassBufs& pb = K.J.pb;
+  const size_t paths = (size_t)n_tiles * R;
+  cudaError_t e = cudaSuccess;
+  pb.bin_start = K.tmp.up(bs.data(), bs.size(), &e);
+  pb.n_slots = K.tmp.up(n_slots.data(), n_slots.size(), &e);
+  pb.q_shade = K.tmp.up(q_shade, (size_t)n_tiles * QS, &e);
+  pb.o_time = reinterpret_cast<float4*>(K.tmp.up(o_time, 4 * paths, &e));
+  pb.d_t = reinterpret_cast<float4*>(K.tmp.up(d_t, 4 * paths, &e));
+  pb.nrm = reinterpret_cast<float4*>(K.tmp.up(nrm, 4 * paths, &e));
+  pb.trap_s = trap ? K.tmp.up(trap_s, paths, &e) : nullptr;
+  pb.prefix_stride = n_tiles + 1;
+  pb.slot_prefix = K.tmp.up<int>(nullptr, (size_t)(1 + RAYN_MAX_HITABLES) * pb.prefix_stride, &e);
+  CU(e);
+  scan_slots_launch(ctx, K.J);
+  normals_launch(ctx, K.J, make_thr(ctx->scene.cam, depth), j);
+  if ((rc = kat_march_end(ctx, K, CNT_EVALS_NORMALS, out_evals))) return rc;
+  CU(cudaMemcpy(nrm, pb.nrm, 4 * paths * sizeof(float), cudaMemcpyDeviceToHost));
+  if (trap) CU(cudaMemcpy(trap_s, pb.trap_s, paths * sizeof(float), cudaMemcpyDeviceToHost));
   return RAYN_OK;
 }

@@ -523,6 +523,48 @@ class Renderer:
                                                 _fptr(nrm0), _fptr(rad), C.byref(p), mp, C.byref(plan)), self._ctx)
         return plan
 
+    def kat_march_extend(self, hk, depth, n_live, q_live, o_time, d_t, q_key, spheres_first=False, paired=False):
+        """k_extend_march of hitable hk over given live rays (include/rayn_b200.h: rayn_b200_kat_march_extend).  n_live int32
+        [n_tiles]; q_live and q_key int32 [n_tiles, R]; o_time and d_t float32 [n_tiles, R, 4].  d_t and q_key are updated in
+        place.  Returns the kernel's distance evaluations."""
+        n_live, q_live = np.ascontiguousarray(n_live, np.int32), np.ascontiguousarray(q_live, np.int32)
+        o_time = np.ascontiguousarray(o_time, np.float32)
+        assert d_t.dtype == np.float32 and q_key.dtype == np.int32 and d_t.flags.c_contiguous and q_key.flags.c_contiguous
+        n_tiles, R = q_live.shape
+        ev = C.c_int64(-1)
+        ip = C.POINTER(C.c_int32)
+        L.check(self._lib.rayn_b200_kat_march_extend(self._ctx, hk, depth, 1 if spheres_first else 0, 1 if paired else 0, n_tiles, R,
+                                                     n_live.ctypes.data_as(ip), q_live.ctypes.data_as(ip), _fptr(o_time), _fptr(d_t),
+                                                     q_key.ctypes.data_as(ip), C.byref(ev)), self._ctx)
+        return ev.value
+
+    def kat_march_shadow(self, j, seg_a, seg_b, vis, paired=False):
+        """k_shadow over a given segment queue of SDF ordinal j (rayn_b200_kat_march_shadow).  seg_a, seg_b float32 [n_seg, 4]
+        (seg_b.w: the bits of owner << 4 | bit); vis uint32 [n_vis], updated in place.  Returns the kernel's distance evaluations."""
+        seg_a, seg_b = np.ascontiguousarray(seg_a, np.float32).reshape(-1, 4), np.ascontiguousarray(seg_b, np.float32).reshape(-1, 4)
+        assert vis.dtype == np.uint32 and vis.flags.c_contiguous
+        ev = C.c_int64(-1)
+        L.check(self._lib.rayn_b200_kat_march_shadow(self._ctx, j, 1 if paired else 0, len(seg_a), _fptr(seg_a), _fptr(seg_b), vis.size,
+                                                     vis.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(ev)), self._ctx)
+        return ev.value
+
+    def kat_march_normals(self, j, depth, bin_start, q_shade, o_time, d_t, nrm, trap_s=None):
+        """k_normals over given shading bins of SDF ordinal j (rayn_b200_kat_march_normals).  bin_start int32 [n_tiles, n_hitables + 1];
+        q_shade int32 [n_tiles, QS]; o_time, d_t float32 [n_tiles, R, 4]; nrm float32 [n_tiles, R, 4] and trap_s float32
+        [n_tiles, R] (materials with an orbit trap) are updated in place.  Returns the kernel's distance evaluations."""
+        bin_start, q_shade = np.ascontiguousarray(bin_start, np.int32), np.ascontiguousarray(q_shade, np.int32)
+        o_time, d_t = np.ascontiguousarray(o_time, np.float32), np.ascontiguousarray(d_t, np.float32)
+        assert nrm.dtype == np.float32 and nrm.flags.c_contiguous
+        assert trap_s is None or (trap_s.dtype == np.float32 and trap_s.flags.c_contiguous)
+        n_tiles, QS = q_shade.shape
+        R = o_time.shape[1]
+        ev = C.c_int64(-1)
+        ip = C.POINTER(C.c_int32)
+        L.check(self._lib.rayn_b200_kat_march_normals(self._ctx, j, depth, n_tiles, R, QS, bin_start.ctypes.data_as(ip), q_shade.ctypes.data_as(ip),
+                                                      _fptr(o_time), _fptr(d_t), _fptr(nrm), None if trap_s is None else _fptr(trap_s),
+                                                      C.byref(ev)), self._ctx)
+        return ev.value
+
     def sdf_variant(self, hitable_index):
         """march-kernel specialisation upload_scene selected for a hitable (include/rayn_b200.h: rayn_b200_debug_sdf_variant)"""
         return int(self._lib.rayn_b200_debug_sdf_variant(self._ctx, hitable_index))
